@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- transition frames/sec of the branch-tree denoising hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one ``BlendingEngine.run_transition()`` of the selected BASELINE.json config (default: configs[1], the
@@ -16,6 +16,8 @@ Prints ONE JSON line (rank 0).  ``value`` = frames/s with the conditioning alrea
 the device; ``e2e`` = the same through the public API (set_prompt1/2 -> run_transition -> PIL frames), host<->device
 copies timed.  ``fingerprint`` = sha1 over the tree (tree_fracts, tree_idx_injection, every branch's final latents):
 equal fingerprints across --gpus 1/2/4/8 mean the sharded run built exactly the single-GPU tree.
+``--dump-outputs DIR`` writes what the last timed step returned as DIR/<name>.npy (see dump_outputs): the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 ``--impl reference`` times the CPU oracle (a port of the reference path: diffusers / lpips are not installable
 here) on the host cores this process may use.
 """
@@ -66,23 +68,15 @@ CONFIGS = {
 
 
 def peaks():
-    p = dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    """Data-sheet peaks of the H100 SXM (dense fp16/bf16 tensor, HBM3) at its 700 W rating; a card with a lower power
+    limit reaches less.  MEASURED_PEAKS.json, when present, replaces them."""
+    p = dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="H100 SXM data sheet")
     fp = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(fp):
         with open(fp) as f:
             p.update(json.load(f))
         p["source"] = "measured"
     return p
-
-
-def measured_traffic():
-    """dram__bytes_read+write per launch from the committed ncu capture (profiles/traffic.json, written by
-    tools/ncu_traffic.py from an `ncu --metrics dram__bytes_*` pass over one UNet forward / one batched mix)."""
-    fp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(fp):
-        with open(fp) as f:
-            return json.load(f)
-    return {}
 
 
 class ClockSampler:
@@ -347,6 +341,26 @@ def tree_fingerprint(be):
     return h.hexdigest()
 
 
+DUMP_FRAME_SAMPLES = 1 << 22      # float32 elements of the frame sample: 16 MB
+
+
+def dump_outputs(out_dir, frames, be):
+    """Write the last timed step's results: ``frames`` (uint8 [n, H, W, 3] stacked and flattened; when larger than
+    DUMP_FRAME_SAMPLES elements, the elements at a fixed seeded sorted sample of flat indices), every branch's final
+    latents (complete) and the tree's mixing fractions.  float32 except tree_fracts (float64); about 21 MB in all."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    flat = torch.stack([f.reshape(-1) for f in frames]).reshape(-1)
+    if flat.numel() > DUMP_FRAME_SAMPLES:
+        idx = np.sort(np.random.default_rng(0).choice(flat.numel(), DUMP_FRAME_SAMPLES, replace=False))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    np.save(os.path.join(out_dir, "frames.npy"), flat.float().cpu().numpy())
+    finals = torch.stack([t[-1] for t in be.tree_latents]).float().cpu().numpy()
+    np.save(os.path.join(out_dir, "final_latents.npy"), finals)
+    np.save(os.path.join(out_dir, "tree_fracts.npy"), np.asarray(be.tree_fracts, dtype=np.float64))
+
+
 def run_ours(args):
     import torch
     rank, local_rank, world = dist_env()
@@ -404,15 +418,18 @@ def run_ours(args):
             ms = float(t)
         return ms / 1e3, n
 
+    last_frames = []
+
     def one_job(api):
         """One bench step.  Configs 2/3/5: one transition.  Config 4: the 8-prompt loop (7 transitions)."""
         be.output_device_frames = not api
+        last_frames.clear()
         if args.config != 4:
             if api:
                 be.set_prompt1(PROMPTS[0])
                 be.set_prompt2(PROMPTS[1])
-            return len(be.run_transition(fixed_seeds=list(cfg["seeds"])))
-        n = 0
+            last_frames.extend(be.run_transition(fixed_seeds=list(cfg["seeds"])))
+            return len(last_frames)
         for i in range(len(PROMPTS_MULTI) - 1):
             if i == 0:
                 be.set_prompt1(PROMPTS_MULTI[0])
@@ -420,8 +437,8 @@ def run_ours(args):
             else:
                 be.swap_forward()
                 be.set_prompt2(PROMPTS_MULTI[i + 1])
-            n += len(be.run_transition(recycle_img1=i > 0, fixed_seeds=[420 + i, 421 + i]))
-        return n
+            last_frames.extend(be.run_transition(recycle_img1=i > 0, fixed_seeds=[420 + i, 421 + i]))
+        return len(last_frames)
 
     for _ in range(max(args.warmup, 0)):
         one_job(False)
@@ -433,6 +450,8 @@ def run_ours(args):
     clocks = sampler.stop()
     fps = frames / sec
     fingerprint = tree_fingerprint(be)          # of the last timed transition (identical every step: fixed seeds)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_frames, be)
     stems_run = [int(v) for v in be.list_nmb_stems]
     # e2e through the public API with host buffers
     one_job(True)
@@ -480,21 +499,17 @@ def run_ours(args):
     gemm_tf = work["gemm_flops"] / (breakdown["gemm"]["ms"] * 1e-3) / 1e12
     attn_tf = work["attn_flops"] / (breakdown["attention"]["ms"] * 1e-3) / 1e12
     norm_gbs = work["norm_bytes"] / max(breakdown["norms"]["ms"] * 1e-3, 1e-9) / 1e9
-    peak_tf, peak_burst = pk["bf16_tflops_sustained"], pk["bf16_tflops"]
-    tr = measured_traffic()
-    roofline = dict(kernel="gemm_tc_kernel (tcgen05 GEMM / implicit-GEMM conv)", bound="tensor", achieved=gemm_tf,
-                    peak=peak_tf, unit="TFLOP/s", frac=gemm_tf / peak_tf, frac_of_burst_peak=gemm_tf / peak_burst,
-                    traffic=tr.get("gemm", {}).get("dram_bytes_per_launch"),
-                    traffic_source=tr.get("gemm", {}).get("source"),
+    peak_tf = pk["bf16_tflops"]
+    roofline = dict(kernel="gemm_tc_kernel (wgmma GEMM / implicit-GEMM conv)", bound="tensor", achieved=gemm_tf,
+                    peak=peak_tf, unit="TFLOP/s", frac=gemm_tf / peak_tf,
                     algorithmic_bytes_per_launch=work["gemm_bytes"] / max(1, breakdown["gemm"]["launches"]),
-                    peak_source=f"{pk['source']} bf16_tflops_sustained (the replay follows minutes of load under the "
-                                f"power cap; burst peak {peak_burst} also given)",
+                    peak_source=pk["source"],
                     algorithmic_flops_per_unet_forward=work["gemm_flops"],
                     avg_launch_us=breakdown["gemm"]["ms"] * 1e3 / max(1, breakdown["gemm"]["launches"]),
                     launches_per_unet_forward=breakdown["gemm"]["launches"],
                     unet_forward_breakdown_ms={k: round(v["ms"], 3) for k, v in breakdown.items()},
                     unet_forward_launches={k: v["launches"] for k, v in breakdown.items()},
-                    attention=dict(kernel="attn_tc_kernel (tcgen05 QK^T / PV, head dim 64)", achieved=attn_tf,
+                    attention=dict(kernel="attn_tc_kernel (wgmma QK^T / PV, head dim 64)", achieved=attn_tf,
                                    frac=attn_tf / peak_tf, flops=work["attn_flops"],
                                    note="all attention launches of one UNet forward incl. cross-attention (77 keys)"),
                     norms=dict(kernel="gn_stats/gn_apply/ln kernels", bound="hbm", achieved=norm_gbs,
@@ -502,9 +517,7 @@ def run_ours(args):
                                algorithmic_bytes=work["norm_bytes"]),
                     mix=dict(kernel="slerp_l2_kernel (K1 parental / crossfeed mix, batched 2048 x 65536 fp16)",
                              bound="hbm", achieved=mix_gbs, peak=pk["hbm_gbs"], unit="GB/s", frac=mix_gbs / pk["hbm_gbs"],
-                             algorithmic_bytes_per_element=6, launch_us=mix_s * 1e6,
-                             traffic=tr.get("mix", {}).get("dram_bytes_per_launch"),
-                             traffic_source=tr.get("mix", {}).get("source")))
+                             algorithmic_bytes_per_element=6, launch_us=mix_s * 1e6))
 
     par = "single GPU" if world == 1 else (f"branch-sharded x{world}: one speculative candidate per rank, CFG halves "
                                            f"split over GPU pairs for the outer trajectories (>= 4 ranks) and the last stems of a level")
@@ -545,6 +558,8 @@ def main():
     ap.add_argument("--t-compute", type=float, default=6.0,
                     help="config 4: t_compute_max_allowed per transition (the reference default is 20 s)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* lb200.h -- C ABI of liblb200.so: the B200-native (sm_100a) backend of the
+/* lb200.h -- C ABI of liblb200.so: the H100-native (sm_90a) backend of the
  * latentblending branch-tree denoising hot path.
  *
  * The reference (lunarring/latentblending @ fd5916a) has no FFI: its operator
@@ -94,7 +94,7 @@ int lb_cfg_euler_step(lb_ctx* ctx, const void* latents_dev, const void* eps_dev,
 
 /* ---- K7 / K4: tensor-core GEMM and implicit-GEMM convolution ----------------
  * out[M,N] = epilogue( conv_taps(a0)[M, taps*a0_c] | a1[M, a1_c] ) x w[N, K]^T ),
- * fp16 operands, fp32 accumulation in TMEM (tcgen05.mma), M = B*H*W rows of an
+ * fp16 operands, fp32 accumulation in registers (wgmma), M = B*H*W rows of an
  * NHWC activation.  taps = 1: Linear / 1x1 conv; taps = 9: 3x3 conv, stride 1,
  * zero padding 1 (weights pre-packed [N][ky][kx][a0_c]).  a1 (optional) is a
  * second 1x1 input appended along K (the resnet shortcut conv folded into
@@ -138,8 +138,8 @@ typedef struct lb_gemm_desc {
  * instead of per 128-row tile; the kernel then runs N = 256 MMAs (fewer shared-memory operand reads per FLOP) */
 #define LB_GEMM_GEGLU256 0x400
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
-/* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per epilogue warp of a
- * TMEM lane quadrant); < 0 on error */
+/* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
+ * that holds a row of the wgmma accumulator); < 0 on error */
 int lb_gemm_stats_parts(lb_ctx* ctx, const lb_gemm_desc* desc);
 
 /* ---- K8: fused attention, head_dim 64 ----------------------------------------

@@ -1,4 +1,4 @@
-"""latentblending_b200: B200-native backend of latentblending's branch-tree
+"""latentblending_b200: H100-native (sm_90a) backend of latentblending's branch-tree
 denoising hot path (BlendingEngine.run_transition -> DiffusersHolder.run_diffusion_sd_xl).
 Same public names as the reference package (latentblending/__init__.py:1-3)."""
 from .utils import add_frames_linear_interp, interpolate_linear, interpolate_spherical  # noqa: F401

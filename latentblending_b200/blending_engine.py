@@ -1,11 +1,11 @@
-"""BlendingEngine: drop-in for latentblending.BlendingEngine on the B200 backend.
+"""BlendingEngine: drop-in for latentblending.BlendingEngine on the H100 backend.
 
 Public surface, defaults and quirks follow latentblending/blending_engine.py
 (:20-96 constructor, :120-293 setters, :295-365 run_transition, :370-465
 compute_latents1/2/_mix, :467-529 get_time_based_branching, :531-588 tree
 placement, :643-654 mixed conditioning, :669-742 writers / swap_forward).
 
-What is different underneath (B200-first, same results):
+What is different underneath (H100-first, same results):
   * the parental mix of a branch (30 per-step slerps in the reference, :442-450)
     is one batched lb_slerp_rows launch over the parents' contiguous trajectory
     slabs (rows where either parent has no latent are simply not computed);
@@ -40,7 +40,7 @@ class BlendingEngine():
             f"guidance_scale_mid_damper neees to be in interval (0,1], you provided {guidance_scale_mid_damper}"
         if do_compile:
             raise ValueError("do_compile selects the reference's stable-fast/Triton path; this backend is already "
-                             "compiled CUDA (sm_100a) and has no such option")
+                             "compiled CUDA (sm_90a) and has no such option")
         self.dh = holder if holder is not None else DiffusersHolder(pipe)
         self.device = self.dh.device
         self.set_dimensions()
@@ -70,9 +70,8 @@ class BlendingEngine():
         self.batch_outer_pair = True          # the two outer trajectories share batch-4 UNet forwards (same results)
         # single-GPU speculation width: candidate branches of a level advanced in lockstep through ONE batched UNet
         # forward (sharding.run_level_local).  None = by model: SDXL-Turbo 512^2 (weight-bandwidth / launch bound, a
-        # batch-4 forward costs about one batch-1 forward) -> 4; SDXL base 1024^2 -> 2 (a batch-4 forward costs 1.78x a
-        # batch-2 one, r02d: worth it while >= 78 % of the second candidates end up in the tree -- the running hit rate
-        # is tracked and the width drops to 1 below that; 13 of 13 on the bench workload, r02e shard stats).
+        # batch-4 forward costs about one batch-1 forward) -> 4; SDXL base 1024^2 -> 2 while >= 78 % of the second
+        # candidates end up in the tree -- the running hit rate is tracked and the width drops to 1 below that.
         self.speculative_batch = None
         self._spec_hits = [0, 0]            # second-or-later candidates: [used, computed], over the engine's lifetime
         # ancestral-scheduler noise per (seeds, branch position, step) from its own generator instead of the global

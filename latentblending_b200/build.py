@@ -1,4 +1,4 @@
-"""Build liblb200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.
+"""Build liblb200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.
 
     python -m latentblending_b200.build        # or __graft_entry__.build()
 
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_build")
 LIB = os.path.join(HERE, "liblb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -64,7 +64,7 @@ def build(verbose=False, force=False):
             if r[2]:
                 print(r[2])
     if rebuilt or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                      "-cudart", "static"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -31,7 +31,7 @@ extern "C" int lb_ctx_create(int device, lb_ctx** out) {
     LB_REQUIRE(device >= 0 && device < count, "lb_ctx_create: device %d out of range (%d devices)", device, count);
     cudaDeviceProp prop;
     LB_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-    LB_REQUIRE(prop.major == 10, "lb_ctx_create: liblb200 is built for sm_100a only; device %d is sm_%d%d",
+    LB_REQUIRE(prop.major == 9 && prop.minor == 0, "lb_ctx_create: liblb200 is built for sm_90a only; device %d is sm_%d%d",
                device, prop.major, prop.minor);
     lb_ctx* c = new lb_ctx();
     c->device = device;

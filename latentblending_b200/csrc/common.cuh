@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for liblb200 (sm_100a only).
+// common.cuh -- shared host/device helpers for liblb200 (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -55,7 +55,7 @@ static inline int64_t lb_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b
 // ---- launches: programmatic dependent launch (PDL) ---------------------------------------------
 // Every kernel of the library is launched with programmatic stream serialization and starts with
 // griddepcontrol.launch_dependents / griddepcontrol.wait: the NEXT kernel's launch latency, block scheduling and
-// prologue (barrier init, TMEM allocation, descriptor prefetch) overlap this kernel's execution; its
+// prologue (barrier init, descriptor prefetch) overlap this kernel's execution; its
 // griddepcontrol.wait returns only when this grid has completed and its writes are visible.
 #ifdef __CUDACC__
 #include <utility>

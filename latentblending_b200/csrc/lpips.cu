@@ -1,7 +1,7 @@
 // lpips.cu -- SURVEY section 8(f) rows #2 and #3 on the device:
 //
 //   #2  LPIPS-AlexNet branch-placement metric (latentblending/blending_engine.py:744-758, lpips==0.1.4 un-vendored):
-//       the five AlexNet convolutions run on the tcgen05 GEMM (lb_gemm with the ReLU epilogue) over patch matrices
+//       the five AlexNet convolutions run on the wgmma GEMM (lb_gemm with the ReLU epilogue) over patch matrices
 //       produced here -- conv1 straight from the uint8 frame with the [-1,1] + ScalingLayer arithmetic fused
 //       (the reference round-trips every frame through PIL and a host->device copy, :750-755) -- plus the 3x3/2
 //       max-pools and the fused "unit-normalise, squared difference, 1x1 lin, spatial mean" tap reduction.

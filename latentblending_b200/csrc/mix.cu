@@ -109,8 +109,8 @@ lerp_kernel(const T* __restrict__ p0, const T* __restrict__ p1, T* __restrict__ 
 }
 
 // fast path launch: cluster of `csize` CTAs per row, `slice` elements of each input per CTA (two passes over
-// global memory, the second served by L2 -- see slerp_l2_kernel).  Tuned on B200 (tools/ubench_mix.cu,
-// profiles/r01c_mix_ubench.txt): 256 threads, 128 elements per thread and input, 4 CTAs resident per SM.
+// global memory, the second served by L2 -- see slerp_l2_kernel).  Tuned with tools/ubench_mix.cu:
+// 256 threads, 128 elements per thread and input, 4 CTAs resident per SM.
 constexpr int kFastThreads = 256;
 constexpr int kFastOcc = 1024;
 constexpr int64_t kSliceElemsTarget = 32768;
@@ -199,7 +199,7 @@ extern "C" int lb_lerp(lb_ctx* ctx, const void* p0, const void* p1, void* out, i
     LB_REQUIRE(dtype == 0 || dtype == 1, "lb_lerp: dtype must be 0 (fp16) or 1 (fp32)");
     const float w0 = (float)(1.0 - fract), w1 = (float)fract;
     unsigned grid = (unsigned)lb_ceil_div(n, kThreads * 4);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > (unsigned)ctx->sm_count * 8) grid = (unsigned)ctx->sm_count * 8;
     if (grid < 1) grid = 1;
     cudaStream_t st = lb_stream(stream);
     if (dtype == 0)

@@ -7,13 +7,13 @@
 //   s0 = sin(theta0 - theta0*f)/sin(theta0); s1 = sin(theta0*f)/sin(theta0);
 //   out = (storage dtype)(float)(p0*s0 + p1*s1)         [fp64 mul, mul, add, no FMA contraction]
 //
-// Two single-DRAM-pass designs live here (both bit-identical to the all-fp64 evaluation; A/B numbers in
-// profiles/r01c_mix_ubench.txt):
+// Two single-DRAM-pass designs live here (both bit-identical to the all-fp64 evaluation; tools/ubench_mix.cu
+// compares them):
 //   slerp_l2_kernel    (the product path): pass 1 streams the row slice from HBM, pass 2 re-reads it from L2.
 //                      No on-chip staging -> ~48 registers, 4-6 CTAs per SM hide the serial section of each CTA
-//                      (row reduction -> cluster exchange -> acos/sin weights).  4.4 TB/s = 67 % of measured HBM.
+//                      (row reduction -> cluster exchange -> acos/sin weights).
 //   slerp_stage_kernel (kept as the measured alternative): cp.async.bulk stages the slice in shared memory once.
-//                      Exact 6 B/elem DRAM traffic, but only 3 CTAs fit per SM: 3.5 TB/s.
+//                      Exact 6 B/elem DRAM traffic, but only 3 CTAs fit per SM.
 // Pass 2 (the axpby): the reference evaluates it in fp64 and rounds fp64 -> fp32 -> fp16; doing that per element
 // costs 3 fp64 conversions + 3 fp64 ops and makes the kernel XU/fp64-pipe-bound (round-1a kernel: 2.1 TB/s).
 // Instead each element is evaluated in packed fp32 with the weights split hi+lo and the fp16 rounding is
@@ -118,20 +118,9 @@ struct SplitW {
 //   below 2^-116; r >= 65520 rounds to inf so d = inf; NaN fails every comparison.  Uncertified elements (~0.1 %)
 //   are recomputed with the reference's fp64 arithmetic, so the output is bit-identical to the all-fp64 evaluation.
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;"
-        : "=l"(reinterpret_cast<uint64_t&>(d))
-        : "l"(reinterpret_cast<const uint64_t&>(a)), "l"(reinterpret_cast<const uint64_t&>(b)),
-          "l"(reinterpret_cast<const uint64_t&>(c)));
-    return d;
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    float2 d;
-    asm("mul.rn.f32x2 %0, %1, %2;"
-        : "=l"(reinterpret_cast<uint64_t&>(d))
-        : "l"(reinterpret_cast<const uint64_t&>(a)), "l"(reinterpret_cast<const uint64_t&>(b)));
-    return d;
-}
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 // scalar form (used by the statistics kernel of tools/ubench_mix.cu; same arithmetic as the packed form)
 __device__ __forceinline__ float slerp_fast(float a, float b, const SplitW& w, float& E) {
     float t = b * w.s1l;
@@ -390,8 +379,8 @@ slerp_stage_kernel(const T* __restrict__ p0, const T* __restrict__ p1, T* __rest
 
 // ---- fast path B: two passes over global memory, the second served by L2 ------------------------
 // No on-chip staging at all: pass 1 streams the CTA's slice of both inputs from HBM (fp64 sums), pass 2 reads the
-// same slice again a few microseconds later -- by then it is resident in the 126 MB L2 (a whole launch keeps
-// < 148 SMs x 8 CTAs x 64 KiB = 76 MB in flight), so DRAM still sees 2 reads + 1 write per element.  With ~40
+// same slice again a few microseconds later -- by then it is resident in L2 (a whole launch keeps
+// < 132 SMs x 8 CTAs x 64 KiB = 68 MB in flight, against the H100's 50 MB L2 the oldest slices may be evicted), so DRAM still sees 2 reads + 1 write per element.  With ~40
 // registers per thread and no shared-memory footprint, 8 CTAs are resident per SM and the long serial section
 // of each CTA (row reduction -> cluster exchange -> acos/sin weights -> second pass) is hidden by the others.
 // The weights are computed ONCE per row (rank 0, warp 0) and broadcast through distributed shared memory.

@@ -97,7 +97,7 @@ gn_partial_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int
         // All 256 threads of the last block combine the chunk partials: thread (slice, g) sums chunks slice, slice + S,
         // ... of group g in fp64 with 8 loads in flight, then the S slices are added in slice order -- a fixed
         // summation order (deterministic, batch-invariant).  One thread per group walking all ~300 chunks was a serial
-        // chain of L2 round trips: ~20 us, most of this kernel's time on the large activations (r02a).
+        // chain of L2 round trips: ~20 us, most of this kernel's time on the large activations.
         __shared__ double f_sum[kThreads], f_sq[kThreads];
         const int S = kThreads / groups;                 // slices (groups <= 64 -> S >= 4)
         const int g = threadIdx.x % groups, slice = threadIdx.x / groups;

@@ -9,7 +9,7 @@
 
 #include <vector>
 
-#include "gemm_sm100.cuh"
+#include "gemm_sm90.cuh"
 
 struct AttnPlan;
 int attn_plan_build_opaque(lb_ctx* ctx, const lb_attn_desc& d, void** plan_out);

@@ -124,7 +124,7 @@ extern "C" int lb_scale_model_input(lb_ctx* ctx, const void* latents, void* out,
     LB_REQUIRE(batch >= 1 && n > 0, "lb_scale_model_input: bad sizes");
     if (n % 8 == 0) LB_REQUIRE(lb_aligned16(latents) && lb_aligned16(out), "lb_scale_model_input: 16-byte alignment");
     unsigned grid = (unsigned)lb_ceil_div(n, n % 8 == 0 ? (int64_t)kThreads * 8 : (int64_t)kThreads);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > (unsigned)ctx->sm_count * 8) grid = (unsigned)ctx->sm_count * 8;
     lb_launch_pdl(scale_input_kernel, grid, kThreads, 0, lb_stream(stream), (const __half*)latents, (__half*)out, n, batch,
                                                                 divisor);
     LB_LAUNCH_CHECK();
@@ -147,7 +147,7 @@ extern "C" int lb_cfg_euler_step(lb_ctx* ctx, const void* latents, const void* e
                        (!scaled_next || lb_aligned16(scaled_next)),
                    "lb_cfg_euler_step: buffers must be 16-byte aligned");
     unsigned grid = (unsigned)lb_ceil_div(n, (int64_t)kThreads * 8);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > (unsigned)ctx->sm_count * 8) grid = (unsigned)ctx->sm_count * 8;
     if (grid < 1) grid = 1;
     const __half* et = eps_text ? (const __half*)eps_text : (const __half*)eps + n;   // default: [2,n] = (uncond, text)
     LB_REQUIRE(n % 8 != 0 || lb_aligned16(et), "lb_cfg_euler_step: eps_text must be 16-byte aligned");

@@ -6,7 +6,7 @@ section 8b): device, pipe, get_text_embedding, get_noise, run_diffusion_sd_xl,
 latent2image, is_sdxl_turbo, set_dimensions, guidance_scale, set_negative_prompt,
 set_num_inference_steps, height_img / width_img.
 
-B200-first differences (results are the same, layout and launch structure are not):
+H100-first differences (results are the same, layout and launch structure are not):
   * a trajectory is ONE contiguous [N,4,h,w] fp16 slab in HBM; the returned
     ``list_latents_out`` holds views into it (None for i < idx_start), so the
     parental mix of a whole branch is a single batched lb_slerp_rows launch;
@@ -57,8 +57,7 @@ class DiffusersHolder:
         self._eps_pair = {}
         # Two CUDA streams for the two CFG halves of a single branch (k = 1): the unconditional and the text half run
         # as two independent batch-1 programs that space-share the SMs, so one half's kernel ramp / drain overlaps the
-        # other's main loop (every kernel is batch-invariant: identical eps).  Measured r02c/r02d on one forward
-        # @128x128: 23.0 ms (one batch-2 program) -> 21.7-22.3 ms.
+        # other's main loop (every kernel is batch-invariant: identical eps).
         self.dual_stream = os.environ.get("LB_DUAL_STREAM", "1") != "0"
         self._dual = {}
 
@@ -148,8 +147,8 @@ class DiffusersHolder:
     @torch.no_grad()
     def run_diffusion_sd_xl_multi(self, jobs, idx_start=0):
         """The denoise loop for k independent branches that share ``idx_start``, advanced in lockstep through ONE
-        UNet forward of batch 2k per step (B200: the 1280-channel levels of a batch-2 SDXL forward are launch- /
-        latency-bound; doubling M is ~17 % cheaper per branch, tools/time_unet_batch.py).  Per branch the arithmetic
+        UNet forward of batch 2k per step (the 1280-channel levels of a batch-2 SDXL forward are launch- /
+        latency-bound, so doubling M costs less than two forwards; tools/time_unet_batch.py measures it).  Per branch the arithmetic
         is exactly run_diffusion_sd_xl's: every kernel on the path is batch-invariant (tests/test_engine_gpu.py).
 
         jobs: dicts with text_embeddings (4-tuple), latents_start, list_latents_mixing, mixing_coeffs and optionally

@@ -4,7 +4,7 @@ Replaces ``lpips.LPIPS(net='alex')`` + ``get_lpips_similarity`` of the reference
 (latentblending/blending_engine.py:74-76, :744-758; lpips==0.1.4, un-vendored): the reference converts both PIL images
 to numpy, copies them to the GPU, scales them to [-1, 1] and runs AlexNet twice per comparison.  Here
   * frames never leave the device (the VAE kernel writes uint8 HWC frames);
-  * the five AlexNet convolutions run on the tcgen05 GEMM (lb_gemm, ReLU epilogue) over patch matrices; conv1's patch
+  * the five AlexNet convolutions run on the wgmma GEMM (lb_gemm, ReLU epilogue) over patch matrices; conv1's patch
     matrix is built straight from the uint8 frame with the [-1,1] + ScalingLayer arithmetic fused (lb_lpips_im2col_u8);
   * the feature stack of a frame is computed ONCE and cached -- every frame of the tree is compared twice or more;
   * a comparison is five fused tap reductions (unit-normalise, squared difference, 1x1 lin, spatial mean).

@@ -9,7 +9,7 @@ tables live on the host; the tensor arithmetic is in csrc/step.cu.
 Scalars are produced with the same fp32 torch expressions the scheduler uses and
 then rounded to fp16 where the reference's CUDA stack rounds them (a 0-dim fp32
 CUDA tensor next to an fp16 tensor is cast to fp16 by PyTorch's binary kernels;
-measured, profiles/r01_probe_scalar_semantics.txt).
+probed by tools/probe_scalar_semantics.py).
 """
 import numpy as np
 import torch

@@ -98,12 +98,10 @@ class LevelSharder:
     # -- teams ---------------------------------------------------------------------------------
     def team_size(self, remaining):
         """Ranks per candidate this round.  A pair (one CFG half per rank) shortens the dependent chain -- a batch-1
-        forward is ~0.72x a batch-2 one (15.7 vs 21.7 ms @128x128, r02d) -- but halves the number of speculative
+        forward costs less than a batch-2 one -- but halves the number of speculative
         candidates per round, and a missed pick costs a whole extra round.  So pairs are used when the pair-teams still
         cover every remaining stem of the level (world // 2 >= remaining: all levels of the 15-branch tree on 8 ranks,
-        the 2- and 1-stem levels on 4 ranks) and for the last stem of a level.  Measured on 4 ranks (r02h): one
-        candidate per rank already finishes every level of the bench tree in ONE round, so more single-rank candidates
-        cannot help 8 ranks -- shorter steps can."""
+        the 2- and 1-stem levels on 4 ranks) and for the last stem of a level."""
         if not self.cfg_pairs:
             return 1
         return 2 if (remaining <= 1 or self.world // 2 >= remaining) else 1

@@ -410,16 +410,14 @@ class UNetB200:
         self.cfg = cfg
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
-        # LayerNorm folding is OFF by default: measured on the same box (r02c, one CFG-batch-2 forward @128x128) 22.98 ms
-        # folded vs 22.40 ms unfused.  The 210 LayerNorm launches need no shared memory, so under PDL they co-reside
-        # with the neighbouring GEMMs' 200 KB CTAs and let the NEXT GEMM's CTAs become resident and prefetch their weights
-        # early; folding them away makes GEMM follow GEMM (no co-residency) and adds epilogue work.  LB_LN_FOLD=1 or
-        # fold_ln=True enables the folded path (same numerics: rel-L2 5.2e-4 either way).
+        # LayerNorm folding is OFF by default: the 210 LayerNorm launches need no shared memory, so under PDL they
+        # co-reside with the neighbouring GEMMs' CTAs; folding them away makes GEMM follow GEMM and adds epilogue work.
+        # LB_LN_FOLD=1 or fold_ln=True enables the folded path (same numerics and tolerance).
         if fold_ln is None:
             fold_ln = os.environ.get("LB_LN_FOLD") is not None
         self.fold_ln = fold_ln
         # GEGLU N tile: 256 (N = 256 MMAs re-read the activation tile half as often) when every FF width allows it;
-        # same-box A/B with the 16-warp epilogue (r02t): 20.35 -> 20.12 ms per forward.  LB_GEGLU_TILE=128 restores 128.
+        # LB_GEGLU_TILE=128 restores 128.
         tile = int(os.environ.get("LB_GEGLU_TILE", "256"))
         widths = [c for c, d in zip(cfg.block_out_channels, cfg.transformer_layers) if d]
         if tile == 256 and any((8 * c) % 256 for c in widths):

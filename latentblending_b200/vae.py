@@ -3,7 +3,7 @@
 Replaces ``pipe.vae.decode(latents / scaling_factor)`` + ``image_processor.postprocess`` inside
 ``DiffusersHolder.latent2image`` (latentblending/diffusers_holder.py:114-143; diffusers 0.25.0
 autoencoder_kl.py / vae.py, un-vendored).  The reference runs the stock SDXL VAE in fp32
-(force_upcast); here the decoder runs in fp16 storage / fp32 accumulation on the same tcgen05
+(force_upcast); here the decoder runs in fp16 storage / fp32 accumulation on the same wgmma
 implicit-GEMM conv, GroupNorm and sampler kernels as the UNet -- 10.5 TFLOP per 1024^2 frame.
 The mid-block single-head attention (head dim 512, S = h*w) is three GEMMs around a row softmax:
 scores = (Wq x)(Wk x)^T (1/sqrt(C) folded into Wq), P = softmax_rows(scores), out = P V with V^T
@@ -190,7 +190,7 @@ class _VAELowering:
         P.groupnorm(x, B, hh * ww, cin, groups, Wt["norm_out.g"], Wt["norm_out.b"], 1e-6, 1, no, self.ws)
         img = torch.empty(1, 3, hh, ww, **f16)
         if Wt.get("conv_out.w8") is not None and os.environ.get("LB_CONV_OUT_DIRECT") is None:
-            # 14 % of a 1024^2 decode went into the direct 128 -> 3 kernel (2.07 ms, r02k); as an N = 8 GEMM it is ~0.2 ms
+            # the direct 128 -> 3 kernel is far slower than the same convolution as an N = 8 GEMM
             P.conv_out_gemm(no, B, hh, ww, cin, Wt["conv_out.w8"], Wt["conv_out.b8"], 3, img, sc("h1", hh * ww, 8))
         else:
             P.conv_out(no, B, hh, ww, cin, Wt["conv_out.w"], Wt["conv_out.b"], 3, img)

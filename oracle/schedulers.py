@@ -16,7 +16,7 @@ All tensor arithmetic is written as individual torch ops on purpose: with fp16
 latents every op rounds to fp16 exactly like the reference stack does, which is
 what the fused CUDA step kernel has to reproduce bit for bit.
 
-Scalar semantics (measured, profiles/r01_probe_scalar_semantics.txt): on the
+Scalar semantics (probed by tools/probe_scalar_semantics.py): on the
 reference's real stack the sigmas live on the CUDA device, and PyTorch's CUDA
 binary kernels cast an fp32 0-dim *CUDA tensor* operand to the fp16 common
 dtype before the fp32 op-math (Python scalars such as guidance_scale stay fp32).

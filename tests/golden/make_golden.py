@@ -1,11 +1,11 @@
-"""Generate golden fixtures by IMPORTING THE REFERENCE (run in the build container
-only; /root/reference does not exist on the GPU box, the tests read the
-committed fixture files).
+"""Generate golden fixtures by IMPORTING THE REFERENCE (a checkout of the original
+latentblending project; the tests read only the committed fixture files).
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path of the latentblending checkout>
 
 * slerp.npz      -- latentblending/utils.py interpolate_spherical / interpolate_linear
-                    outputs on seeded inputs (fp16 and fp32, several fracts incl. 0/1).
+                    outputs on the seeded inputs of slerp_cases.py (fp16 and fp32,
+                    several fracts incl. 0/1); the inputs are regenerated, not stored.
 * tree.json      -- the reference BlendingEngine host logic (run_transition,
                     get_mixing_parameters, insert_into_tree, compute_latents_mix
                     coefficient schedules, set_guidance_mid_dampening,
@@ -25,7 +25,6 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-REF = "/root/reference"
 
 
 def _stub(name, **attrs):
@@ -36,7 +35,7 @@ def _stub(name, **attrs):
     return m
 
 
-def import_reference():
+def import_reference(ref):
     _stub("lpips", LPIPS=object)
     _stub("lunar_tools", MovieSaver=object, fill_up_frames_linear_interpolation=None)
     _stub("diffusers", DiffusionPipeline=object, StableDiffusionControlNetPipeline=object, ControlNetModel=object)
@@ -46,30 +45,19 @@ def import_reference():
     _stub("diffusers.pipelines")
     _stub("diffusers.pipelines.stable_diffusion_xl")
     _stub("diffusers.pipelines.stable_diffusion_xl.pipeline_stable_diffusion_xl", retrieve_timesteps=None)
-    sys.path.insert(0, REF)
+    sys.path.insert(0, ref)
     import latentblending.utils as ref_utils
     import latentblending.blending_engine as ref_engine
     return ref_utils, ref_engine
 
 
 def golden_slerp(ref_utils):
+    from slerp_cases import slerp_inputs
     out = {}
-    g = torch.Generator().manual_seed(1234)
-    cases = []
-    for n, dt in ((64, torch.float16), (4 * 16 * 16, torch.float16), (4 * 64 * 64, torch.float16),
-                  (4 * 128 * 128, torch.float16), (777, torch.float32)):
-        for f in (0.0, 0.25, 0.5, 0.3141, 1.0):
-            cases.append((n, dt, f))
-    for k, (n, dt, f) in enumerate(cases):
-        p0 = (torch.randn(n, generator=g) * (1 + k % 3)).to(dt)
-        p1 = (torch.randn(n, generator=g) * 2).to(dt)
-        if k % 7 == 3:
-            p1 = (p0.float() * 1.5).to(dt)          # parallel vectors -> exercises the 1e-7 clamp
-        r = ref_utils.interpolate_spherical(p0, p1, f)
-        out[f"p0_{k}"] = p0.numpy()
-        out[f"p1_{k}"] = p1.numpy()
+    cases, g = slerp_inputs()
+    for k, (p0, p1, f) in enumerate(cases):
         out[f"f_{k}"] = np.float64(f)
-        out[f"out_{k}"] = r.numpy()
+        out[f"out_{k}"] = ref_utils.interpolate_spherical(p0, p1, f).numpy()
     out["n_cases"] = np.int64(len(cases))
     # interpolate_linear on tensors and uint8 frames
     a = torch.randn(1, 77, 64, generator=g).half()
@@ -177,6 +165,6 @@ def golden_tree(ref_engine):
 
 
 if __name__ == "__main__":
-    ref_utils, ref_engine = import_reference()
+    ref_utils, ref_engine = import_reference(sys.argv[1])
     golden_slerp(ref_utils)
     golden_tree(ref_engine)

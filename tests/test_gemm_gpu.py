@@ -1,4 +1,4 @@
-"""GPU numerics: the tcgen05 GEMM / implicit-GEMM conv kernel (lb_gemm) against a
+"""GPU numerics: the wgmma GEMM / implicit-GEMM conv kernel (lb_gemm) against a
 plain PyTorch fp32 reference of the same op on the same fp16 inputs.
 Tolerance: fp16 storage of an fp32-accumulated result -> |err| <= 2e-3*|ref|_max + small abs."""
 import pytest

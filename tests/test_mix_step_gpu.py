@@ -13,11 +13,13 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 def test_slerp_golden_bit_exact():
     from latentblending_b200 import utils
+    from slerp_cases import slerp_inputs
     z = np.load(os.path.join(GOLD, "slerp.npz"))
-    for k in range(int(z["n_cases"])):
-        p0 = torch.from_numpy(z[f"p0_{k}"]).cuda()
-        p1 = torch.from_numpy(z[f"p1_{k}"]).cuda()
-        out = utils.interpolate_spherical(p0, p1, float(z[f"f_{k}"])).cpu()
+    cases, _ = slerp_inputs()
+    assert len(cases) == int(z["n_cases"])
+    for k, (p0, p1, f) in enumerate(cases):
+        assert f == float(z[f"f_{k}"])
+        out = utils.interpolate_spherical(p0.cuda(), p1.cuda(), f).cpu()
         ref = torch.from_numpy(z[f"out_{k}"])
         assert out.dtype == ref.dtype
         assert torch.equal(out, ref), f"case {k}: {(out != ref).sum().item()} mismatches"

@@ -17,10 +17,13 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def test_slerp_matches_reference_golden():
+    from slerp_cases import slerp_inputs
     z = np.load(os.path.join(GOLD, "slerp.npz"))
-    for k in range(int(z["n_cases"])):
-        p0, p1 = torch.from_numpy(z[f"p0_{k}"]), torch.from_numpy(z[f"p1_{k}"])
-        out = mixing.interpolate_spherical(p0, p1, float(z[f"f_{k}"]))
+    cases, _ = slerp_inputs()
+    assert len(cases) == int(z["n_cases"])
+    for k, (p0, p1, f) in enumerate(cases):
+        assert f == float(z[f"f_{k}"])
+        out = mixing.interpolate_spherical(p0, p1, f)
         ref = torch.from_numpy(z[f"out_{k}"])
         assert out.dtype == ref.dtype
         assert torch.equal(out, ref), f"case {k}"

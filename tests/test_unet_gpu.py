@@ -1,10 +1,10 @@
 """GPU parity of the lowered UNet program (liblb200) against the CPU oracle UNet
 (oracle/sdxl_unet.py, fp32) on identical seeded weights and inputs.
 Tolerance (stated): relative L2 error of eps <= 2e-3 (SURVEY section 8c) -- fp16 storage of every
-activation with fp32 accumulation vs an all-fp32 oracle; measured 5.0e-4 ... 5.2e-4 (r02a).  At the BENCHMARKED shape
+activation with fp32 accumulation vs an all-fp32 oracle.  At the BENCHMARKED shape
 (full SDXL-base, CFG batch 2, 128x128 latents) the comparison is against the committed
 fixture tests/golden/unet_sdxl_b2_128.npz (tests/golden/make_fullsize_fixtures.py).
-Measured rel-L2 values are printed (-s) and recorded in DESIGN.md section 5."""
+Measured rel-L2 values are printed (-s)."""
 import dataclasses
 
 import pytest

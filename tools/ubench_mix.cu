@@ -1,5 +1,5 @@
 // ubench_mix.cu -- stand-alone micro-benchmark / A-B check of the K1 slerp kernels (no torch, no liblb200).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo tools/ubench_mix.cu -o tools/ubench_mix
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo tools/ubench_mix.cu -o tools/ubench_mix
 // V0   = round-1a register-resident cluster kernel (kept here only as the baseline and bit-exactness anchor:
 //        it is the kernel the pytest parity suite validated against the torch oracle)
 // S<T> = slerp_stage_kernel<__half, T, exact?> from latentblending_b200/csrc/mix_kernels.cuh
