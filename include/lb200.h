@@ -134,9 +134,6 @@ typedef struct lb_gemm_desc {
 #define LB_GEMM_STATIC_W 0x100
 /* mode flag (linear epilogue): out = max(out, 0) -- the AlexNet convolutions of the LPIPS metric */
 #define LB_GEMM_RELU 0x200
-/* mode flag (GEGLU): the weight rows are interleaved per 256-row tile (128 value rows, then their 128 gate rows)
- * instead of per 128-row tile; the kernel then runs N = 256 MMAs (fewer shared-memory operand reads per FLOP) */
-#define LB_GEMM_GEGLU256 0x400
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
 /* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
  * that holds a row of the wgmma accumulator); < 0 on error */

@@ -95,7 +95,6 @@ class Op(ctypes.Structure):
 
 GEMM_STATIC_W = 0x100     # lb_gemm_desc.mode flag (include/lb200.h: LB_GEMM_STATIC_W)
 GEMM_RELU = 0x200         # LB_GEMM_RELU
-GEMM_GEGLU256 = 0x400     # LB_GEMM_GEGLU256
 (OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN, OP_CONV_OUT,
  OP_UPSAMPLE2X, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
  OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = range(1, 18)

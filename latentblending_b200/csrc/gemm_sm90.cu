@@ -12,12 +12,18 @@
 //
 // Structure (one CTA per SM, persistent over 128 x BN output tiles, 384 threads = three warpgroups):
 //   warpgroup 0   : TMA producer -- one warp issues cp.async.bulk.tensor 4D (A) / 2D (W) into a STAGES-deep
-//                   128B-swizzled smem ring, mbarrier full/empty pairs; the warpgroup gives its registers away
-//   warpgroups 1-2: consumers    -- each owns 64 rows of the tile: wgmma.m64nBNk16 (fp16 in, fp32 accumulators in
-//                   registers, one k-block in flight while the previous one's slot is released), then the
-//                   epilogue straight from the accumulators: + bias / per-batch bias (time embedding) / residual,
-//                   or GEGLU, or the LayerNorm fold, fp16 store.  The producer runs ahead into the next tile's
-//                   k-blocks while the consumers drain the epilogue.
+//                   128B-swizzled smem ring, mbarrier full/empty pairs, in the CTA's tile order; the warpgroup gives
+//                   its registers away
+//   warpgroups 1-2: consumers, ping-pong -- each owns whole 128-row tiles, alternating through the CTA's tiles
+//                   (warpgroup 1: tiles 0, 2, 4, ...; warpgroup 2: tiles 1, 3, 5, ...).  Per k16 step two
+//                   wgmma.m64nBNk16 (rows 0-63 and 64-127) share the B descriptor; fp16 in, fp32 accumulators in
+//                   registers, one k-block in flight while the previous one's slot is released.  A pair of
+//                   mbarriers lets one warpgroup at a time issue its main loop; the other meanwhile runs its epilogue
+//                   straight from the accumulators: + bias / per-batch bias (time embedding) / residual, or GEGLU,
+//                   or the LayerNorm fold, fp16 store.  So the tensor pipe keeps working through every epilogue
+//                   but a CTA's last.
+//                   BN = 256 (long-K convolutions only, see gemm_plan_build) does not fit one warpgroup's registers
+//                   at 128 rows: there both warpgroups work on every tile, 64 rows each (cooperative).
 // Weight (B operand) tiles of the first pipeline stages are requested BEFORE
 // griddepcontrol.wait when the caller marks the weights static (LB_GEMM_STATIC_W):
 // their HBM latency hides behind the tail of the previous kernel.
@@ -36,13 +42,18 @@ constexpr int kBK = 64;
 constexpr int kEpiParts = 4;                 // stats_out partial sums per row and N tile: one per lane of a quad
 constexpr int kThreadsGemm = 384;            // warpgroup 0 TMA, warpgroups 1-2 wgmma + epilogue
 constexpr int kABytes = kBM * kBK * 2;  // 16 KiB
+constexpr int kGegluBN = 128;                // N tile of GEGLU launches (64 value + 64 gate columns)
 
 template <int BN> struct Cfg {
     static constexpr int b_bytes = BN * kBK * 2;
     static constexpr int stage_bytes = kABytes + b_bytes;
-    // ring depth (GemmParams::stages): as many stages as 227 KB of shared memory allow
-    static constexpr int deep = (BN <= 64) ? 8 : (BN <= 128) ? 7 : (BN <= 160) ? 6 : 4;
-    static constexpr int smem_bytes(int nst) { return nst * stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/; }
+    // ring depth: as many stages as 227 KB of shared memory allow
+    static constexpr int stages = (BN <= 64) ? 8 : (BN <= 128) ? 7 : (BN <= 160) ? 6 : 4;
+    // consumer schedule: ping-pong over whole tiles while a warpgroup's BN fp32 accumulators per thread fit its 232
+    // registers (BN <= 160); cooperative (64 rows per warpgroup) for BN = 256
+    static constexpr bool coop = BN > 160;
+    static constexpr int smem_bytes = stages * stage_bytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(smem_bytes <= 227 * 1024, "smem ring does not fit");
 };
 
 // exact-erf GELU, 0.5 x (1 + erf(x / sqrt 2)), with erf from Abramowitz & Stegun 7.1.26 (|error| <= 1.5e-7, far below
@@ -61,10 +72,8 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return 0.5f * x * one_plus_erf;
 }
 
-__device__ __forceinline__ float2 ld_h2(const __half* p) {
-    return __half22float2(__ldg(reinterpret_cast<const __half2*>(p)));
-}
 __device__ __forceinline__ float2 ld_f2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
+__device__ __forceinline__ __half2 ld_h2(const __half* p) { return __ldg(reinterpret_cast<const __half2*>(p)); }
 
 // (mu, rstd) of one row of the LayerNorm-folded A operand from the producer's per-row partial sums (fixed order).
 // The partials of a row are contiguous (<= 64 x float2): they are fetched as float4 pairs, eight loads in flight at
@@ -94,19 +103,180 @@ __device__ __forceinline__ void ln_row_stats(const GemmParams& p, long long row,
     rstd = rsqrtf((float)var + p.ln_eps);
 }
 
+// One accumulator row of the current tile as the epilogue sees it.
+struct EpiRow {
+    long long row;     // output row (pixel index b*H*W + y*W + x)
+    int bidx;          // batch index (bias2 row)
+    bool ok;           // inside the output
+    float ln_mu, ln_rstd;
+};
+
+// Epilogues of one 64-row half of the tile.  The thread holds rows r[0], r[1] (acc[4j + 2i + e] is row r[i], column
+// 8j + 2*quad + e).  The global loads of a batch of column groups are all issued before any of its stores: the
+// residual may alias the output (in-place `hs += f(hs)`) and only this thread reads and writes these elements, so
+// the order is safe, and the loads overlap instead of costing one L2 round trip per 8-column group.
+template <int BN>
+__device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float (&acc)[BN / 2], const EpiRow (&r)[2],
+                                                int n_tile, int quad) {
+    constexpr int G = BN / 8;                    // 8-column groups per row
+    constexpr int CH = G > 10 ? G / 2 : G;       // groups per load batch (register budget)
+    static_assert(G % CH == 0, "load batches must tile the row");
+    const int n_base = n_tile * BN + 2 * quad;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        if (!r[i].ok) continue;
+        float st_sum = 0.f, st_sq = 0.f;
+        const __half* res_row = p.res ? p.res + r[i].row * p.ldr : nullptr;
+        const __half* b2_row = p.bias2 ? p.bias2 + (long long)r[i].bidx * p.bias2_ld : nullptr;
+        __half* out_row = p.out + r[i].row * p.ldo;
+#pragma unroll
+        for (int c0 = 0; c0 < G; c0 += CH) {
+            float v[CH][2];
+#pragma unroll
+            for (int g = 0; g < CH; ++g) {
+                v[g][0] = acc[4 * (c0 + g) + 2 * i];
+                v[g][1] = acc[4 * (c0 + g) + 2 * i + 1];
+            }
+            if (p.ln_stats) {
+                constexpr int CL = CH > 8 ? CH / 2 : CH;     // fp32 vectors: half the batch
+#pragma unroll
+                for (int l0 = 0; l0 < CH; l0 += CL) {
+                    float2 c[CL], t[CL];
+#pragma unroll
+                    for (int g = 0; g < CL; ++g) {
+                        const int n = n_base + 8 * (c0 + l0 + g);
+                        c[g] = n < p.N ? ld_f2(p.ln_csum + n) : make_float2(0.f, 0.f);
+                        t[g] = n < p.N ? ld_f2(p.ln_bias + n) : make_float2(0.f, 0.f);
+                    }
+#pragma unroll
+                    for (int g = 0; g < CL; ++g) {
+                        v[l0 + g][0] = fmaf(r[i].ln_rstd, v[l0 + g][0] - r[i].ln_mu * c[g].x, t[g].x);
+                        v[l0 + g][1] = fmaf(r[i].ln_rstd, v[l0 + g][1] - r[i].ln_mu * c[g].y, t[g].y);
+                    }
+                }
+            } else {
+                const __half2 z = __float2half2_rn(0.f);
+                __half2 hb[CH], hb2[CH], hr[CH];
+#pragma unroll
+                for (int g = 0; g < CH; ++g) {
+                    const int n = n_base + 8 * (c0 + g);    // N is a multiple of 8 (checked on the host)
+                    const bool in = n < p.N;
+                    hb[g] = (p.bias && in) ? ld_h2(p.bias + n) : z;
+                    hb2[g] = (b2_row && in) ? ld_h2(b2_row + n) : z;
+                    hr[g] = (res_row && in) ? *reinterpret_cast<const __half2*>(res_row + n) : z;
+                }
+#pragma unroll
+                for (int g = 0; g < CH; ++g) {
+                    if (p.bias) {
+                        const float2 t = __half22float2(hb[g]);
+                        v[g][0] += t.x;
+                        v[g][1] += t.y;
+                    }
+                    if (b2_row) {
+                        const float2 t = __half22float2(hb2[g]);
+                        v[g][0] += t.x;
+                        v[g][1] += t.y;
+                    }
+                    if (res_row) {
+                        const float2 t = __half22float2(hr[g]);
+                        v[g][0] += t.x;
+                        v[g][1] += t.y;
+                    }
+                }
+            }
+#pragma unroll
+            for (int g = 0; g < CH; ++g) {
+                const int n = n_base + 8 * (c0 + g);
+                if (n < p.N) {
+                    float v0 = v[g][0], v1 = v[g][1];
+                    if (p.relu) {
+                        v0 = fmaxf(v0, 0.f);
+                        v1 = fmaxf(v1, 0.f);
+                    }
+                    const __half2 o = __floats2half2_rn(v0, v1);
+                    *reinterpret_cast<__half2*>(out_row + n) = o;
+                    if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
+                        const float2 f = __half22float2(o);
+                        st_sum += f.x + f.y;
+                        st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
+                    }
+                }
+            }
+        }
+        if (p.stats_out)
+            p.stats_out[r[i].row * (kEpiParts * p.tiles_n) + kEpiParts * n_tile + quad] = make_float2(st_sum, st_sq);
+    }
+}
+
+// GEGLU: tile columns [0,BN/2) are "value", [BN/2,BN) the matching "gate" (weights are row-interleaved per tile on
+// the host); out = (v+bv) * gelu(g+bg), BN/2 outputs per tile.
+template <int BN>
+__device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float (&acc)[BN / 2], const EpiRow (&r)[2],
+                                               int n_tile, int quad) {
+    constexpr int HN = BN / 2;
+    constexpr int G = HN / 8;
+    const int o_base = n_tile * HN + 2 * quad;     // output column base
+    const int a_base = n_tile * BN + 2 * quad;     // accumulator (bias) column base
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        if (!r[i].ok) continue;
+        __half* out_row = p.out + r[i].row * p.ldo;
+        float2 bv[G], bg[G];
+        if (p.ln_stats) {
+            float2 cv[G], cg[G];
+#pragma unroll
+            for (int j = 0; j < G; ++j) {
+                cv[j] = ld_f2(p.ln_csum + a_base + 8 * j);
+                cg[j] = ld_f2(p.ln_csum + a_base + HN + 8 * j);
+                bv[j] = ld_f2(p.ln_bias + a_base + 8 * j);
+                bg[j] = ld_f2(p.ln_bias + a_base + HN + 8 * j);
+            }
+#pragma unroll
+            for (int j = 0; j < G; ++j) {
+                float v[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
+                float g[2] = {acc[4 * (j + G) + 2 * i], acc[4 * (j + G) + 2 * i + 1]};
+                v[0] = r[i].ln_rstd * (v[0] - r[i].ln_mu * cv[j].x);
+                v[1] = r[i].ln_rstd * (v[1] - r[i].ln_mu * cv[j].y);
+                g[0] = r[i].ln_rstd * (g[0] - r[i].ln_mu * cg[j].x);
+                g[1] = r[i].ln_rstd * (g[1] - r[i].ln_mu * cg[j].y);
+                // the reference rounds proj output, gelu(gate) and the product to fp16
+                const float r0 = lb_round_h(v[0] + bv[j].x) * lb_round_h(gelu_erf(lb_round_h(g[0] + bg[j].x)));
+                const float r1 = lb_round_h(v[1] + bv[j].y) * lb_round_h(gelu_erf(lb_round_h(g[1] + bg[j].y)));
+                *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < G; ++j) {
+                bv[j] = p.bias ? __half22float2(ld_h2(p.bias + a_base + 8 * j)) : make_float2(0.f, 0.f);
+                bg[j] = p.bias ? __half22float2(ld_h2(p.bias + a_base + HN + 8 * j)) : make_float2(0.f, 0.f);
+            }
+#pragma unroll
+            for (int j = 0; j < G; ++j) {
+                const float r0 = lb_round_h(acc[4 * j + 2 * i] + bv[j].x) *
+                                 lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i] + bg[j].x)));
+                const float r1 = lb_round_h(acc[4 * j + 2 * i + 1] + bv[j].y) *
+                                 lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i + 1] + bg[j].y)));
+                *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
+            }
+        }
+    }
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
     using C = Cfg<BN>;
+    constexpr int nst = C::stages;
+    constexpr bool kCoop = C::coop;
     pdl_launch_dependents();       // the next kernel may start its launch + prologue while this one runs
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_addr = smem_u32(smem_raw);
     uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);  // SWIZZLE_128B needs 1024 B alignment
     uint8_t* smem_a = smem;
-    const int nst = p.stages;      // ring depth (Cfg::deep)
     uint8_t* smem_b = smem + nst * kABytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + nst * C::stage_bytes);
     uint64_t* full = bars;
     uint64_t* empty = bars + nst;
+    uint64_t* turn = bars + 2 * nst;   // ping-pong: turn[c] completes when consumer warpgroup c may issue its main loop
 
     const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
     const int wg = warp >> 2;
@@ -117,8 +287,10 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
         tma_prefetch_desc(&p.tmB);
         for (int s = 0; s < nst; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 2);       // one arrive per consumer warpgroup
+            mbar_init(&empty[s], kCoop ? 2 : 1);       // released by every warpgroup that consumed the slot
         }
+        mbar_init(&turn[0], 128);                        // every thread of the other warpgroup arrives
+        mbar_init(&turn[1], 128);
         fence_mbar_init();
     }
     __syncthreads();
@@ -148,6 +320,7 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
         reg_dealloc<40>();
         if (warp != 0) return;
         // ===================== TMA producer (whole warp runs the loop, one elected lane issues) =====================
+        // The ring holds the CTA's tiles in order, which is the order the two consumer warpgroups take turns in.
         int stage = 0;
         uint32_t phase = 0;
         for (int tile = tile0; tile < num_tiles; tile += tile_step) {
@@ -179,145 +352,114 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
         return;
     }
 
-    // ===================== consumers: warpgroup 1 rows [0,64), warpgroup 2 rows [64,128) of the tile =====================
+    // ===================== consumers
+    // ping-pong (BN <= 160): warpgroup 1 takes the CTA's tiles 0, 2, 4, ..., warpgroup 2 tiles 1, 3, 5, ..., each
+    //   computes all 128 rows of its tile;
+    // cooperative (BN = 256, whose 128-row tile would not fit one warpgroup's registers): both take every tile,
+    //   warpgroup 1 rows 0-63, warpgroup 2 rows 64-127.
     reg_alloc<232>();
     const int cw = wg - 1;
     const bool wg_leader = (threadIdx.x & 127) == 0;
     const int quad = lane & 3;
-    int rr[2], ww[2], hh[2], bb[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        rr[i] = cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;      // accumulator row inside the 128-row tile
-        ww[i] = rr[i] % p.tw;
-        hh[i] = (rr[i] / p.tw) % p.th;
-        bb[i] = rr[i] / (p.tw * p.th);
-    }
-    float acc[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+    const int my_tiles = tile0 < num_tiles ? (num_tiles - tile0 + tile_step - 1) / tile_step : 0;
+    constexpr int kHalves = kCoop ? 1 : 2;   // 64-row halves of the tile this warpgroup computes
+    float acc[kHalves][BN / 2];
+    const auto half_of = [&](int hh) { return kCoop ? cw : hh; };
+    for (int j = kCoop ? 0 : cw; j < my_tiles; j += kCoop ? 1 : 2) {
+        const int tile = tile0 + j * tile_step;
         const int m_tile = tile % m_groups, n_tile = tile / m_groups;
-        bool row_ok[2];
-        long long row[2];
-        int bidx[2];
-        float ln_mu[2] = {0.f, 0.f}, ln_rstd[2] = {1.f, 1.f};
+        // this thread's accumulator rows inside the 128-row tile: 64h + 16*(warp%4) + lane/4 + 8i is er[hh][i]
+        EpiRow er[kHalves][2];
+        const auto row_of = [&](int hh, int i) {
+            const int rr = half_of(hh) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+            const int x = (m_tile % p.tiles_x) * p.tw + rr % p.tw;
+            const int y = ((m_tile / p.tiles_x) % p.tiles_y) * p.th + (rr / p.tw) % p.th;
+            const int b = (m_tile / (p.tiles_x * p.tiles_y)) * p.tb + rr / (p.tw * p.th);
+            EpiRow& e = er[hh][i];
+            e.ok = (x < p.W) && (y < p.H) && (b < p.B);
+            e.row = ((long long)b * p.H + y) * p.W + x;
+            e.bidx = b;
+        };
+        // LayerNorm-fold row statistics: fetched before the main loop so their latency hides behind it
+        float ln_mu[kHalves][2], ln_rstd[kHalves][2];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int x = (m_tile % p.tiles_x) * p.tw + ww[i];
-            const int y = ((m_tile / p.tiles_x) % p.tiles_y) * p.th + hh[i];
-            const int b = (m_tile / (p.tiles_x * p.tiles_y)) * p.tb + bb[i];
-            row_ok[i] = (x < p.W) && (y < p.H) && (b < p.B);
-            row[i] = ((long long)b * p.H + y) * p.W + x;
-            bidx[i] = b;
-            if (p.ln_stats) ln_row_stats(p, row[i], row_ok[i], ln_mu[i], ln_rstd[i]);
+        for (int hh = 0; hh < kHalves; ++hh)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                ln_mu[hh][i] = 0.f;
+                ln_rstd[hh][i] = 1.f;
+                if (p.ln_stats) {
+                    row_of(hh, i);
+                    ln_row_stats(p, er[hh][i].row, er[hh][i].ok, ln_mu[hh][i], ln_rstd[hh][i]);
+                }
+            }
+        // this tile's k-blocks follow the j tiles before it in the ring
+        const uint32_t it0 = (uint32_t)j * (uint32_t)p.total_kb;
+        int stage = (int)(it0 % nst);
+        uint32_t phase = (it0 / nst) & 1u;
+        // The first wgmma ignores the accumulators' values; zeroing them anyway ends the previous tile's values at
+        // its epilogue, so the epilogue may reuse their registers.
+#pragma unroll
+        for (int hh = 0; hh < kHalves; ++hh)
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[hh][i] = 0.f;
+        // ---- main loop; in ping-pong, issued only once the other warpgroup has issued all of tile j - 1.  That
+        // order also keeps every full[] barrier at most one phase behind the one this warpgroup waits for.
+        // Tile j > 0 waits for completion (j - 1) / 2 of turn[cw] (the other warpgroup's tiles j - 1, j + 1, ...);
+        // a bounded wait, so a protocol error traps instead of hanging the GPU.
+        if (!kCoop && j > 0) {      // (the branch keeps the barrier address a compile-time offset)
+            const uint32_t par = (uint32_t)((j - 1) >> 1) & 1u;
+            if (cw == 0) mbar_wait(&turn[0], par, p.err_flag, 4);
+            else mbar_wait(&turn[1], par, p.err_flag, 4);
         }
-        // ---- main loop: one k-block of wgmmas in flight; the slot of the previous k-block is released once done
         int prev_stage = -1;
         for (int kb = 0; kb < p.total_kb; ++kb) {
             mbar_wait(&full[stage], phase, p.err_flag, 3);
-            const uint32_t a_addr = smem_u32(smem_a + stage * kABytes) + cw * (64 * 128);
+            const uint32_t a_addr = smem_u32(smem_a + stage * kABytes);
             const uint32_t b_addr = smem_u32(smem_b + stage * C::b_bytes);
-            fence_regs(acc);
+#pragma unroll
+            for (int hh = 0; hh < kHalves; ++hh) fence_regs(acc[hh]);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kBK / 16; ++k)
-                WgmmaSS<BN>::template mma<0>(acc, make_smem_desc_sw128(a_addr + k * 32, 16, 1024),
-                                             make_smem_desc_sw128(b_addr + k * 32, 16, 1024), (kb | k) != 0);
+            for (int k = 0; k < kBK / 16; ++k) {
+                const uint64_t bdesc = make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
+#pragma unroll
+                for (int hh = 0; hh < kHalves; ++hh)
+                    WgmmaSS<BN>::template mma<0>(acc[hh],
+                                                 make_smem_desc_sw128(a_addr + half_of(hh) * (64 * 128) + k * 32, 16,
+                                                                      1024),
+                                                 bdesc, (kb | k) != 0);
+            }
             wgmma_commit();
             wgmma_wait<1>();
-            fence_regs(acc);
+#pragma unroll
+            for (int hh = 0; hh < kHalves; ++hh) fence_regs(acc[hh]);
             if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
             prev_stage = stage;
             if (++stage == nst) { stage = 0; phase ^= 1; }
         }
+        if (!kCoop && j + 1 < my_tiles) {     // the other warpgroup's turn
+            if (cw == 0) mbar_arrive(&turn[1]);
+            else mbar_arrive(&turn[0]);
+        }
         wgmma_wait<0>();
-        fence_regs(acc);
+#pragma unroll
+        for (int hh = 0; hh < kHalves; ++hh) fence_regs(acc[hh]);
         if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
+#pragma unroll
+        for (int hh = 0; hh < kHalves; ++hh)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                row_of(hh, i);
+                er[hh][i].ln_mu = ln_mu[hh][i];
+                er[hh][i].ln_rstd = ln_rstd[hh][i];
+            }
 
-        // ---- epilogue from registers: this thread holds rows rr[0], rr[1] and columns 8j + 2*quad + {0, 1}
-        if (p.mode == 0) {
-            const int n_base = n_tile * BN + 2 * quad;
+        // ---- epilogue from registers (in ping-pong, overlapping the other warpgroup's main loop)
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                float st_sum = 0.f, st_sq = 0.f;
-                if (row_ok[i]) {
-                    const __half* res_row = p.res ? p.res + row[i] * p.ldr : nullptr;
-                    __half* out_row = p.out + row[i] * p.ldo;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int n = n_base + 8 * j;
-                        if (n < p.N) {        // N is a multiple of 8 (checked on the host)
-                            float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-                            if (p.ln_stats) {
-                                const float2 c = ld_f2(p.ln_csum + n), t = ld_f2(p.ln_bias + n);
-                                v0 = fmaf(ln_rstd[i], v0 - ln_mu[i] * c.x, t.x);
-                                v1 = fmaf(ln_rstd[i], v1 - ln_mu[i] * c.y, t.y);
-                            } else if (p.bias) {
-                                const float2 t = ld_h2(p.bias + n);
-                                v0 += t.x;
-                                v1 += t.y;
-                            }
-                            if (p.bias2) {
-                                const float2 t = ld_h2(p.bias2 + (long long)bidx[i] * p.bias2_ld + n);
-                                v0 += t.x;
-                                v1 += t.y;
-                            }
-                            if (res_row) {
-                                const float2 t = __half22float2(*reinterpret_cast<const __half2*>(res_row + n));
-                                v0 += t.x;
-                                v1 += t.y;
-                            }
-                            if (p.relu) {
-                                v0 = fmaxf(v0, 0.f);
-                                v1 = fmaxf(v1, 0.f);
-                            }
-                            const __half2 o = __floats2half2_rn(v0, v1);
-                            *reinterpret_cast<__half2*>(out_row + n) = o;
-                            if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
-                                const float2 f = __half22float2(o);
-                                st_sum += f.x + f.y;
-                                st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
-                            }
-                        }
-                    }
-                    if (p.stats_out)
-                        p.stats_out[row[i] * (kEpiParts * p.tiles_n) + kEpiParts * n_tile + quad] =
-                            make_float2(st_sum, st_sq);
-                }
-            }
-        } else {
-            // GEGLU: tile columns [0,BN/2) are "value", [BN/2,BN) the matching "gate" (weights are
-            // row-interleaved per tile on the host); out = (v+bv) * gelu(g+bg), BN/2 outputs per tile.
-            constexpr int HN = BN / 2;
-            const int o_base = n_tile * HN + 2 * quad;     // output column base
-            const int a_base = n_tile * BN + 2 * quad;     // accumulator (bias) column base
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                if (!row_ok[i]) continue;
-                __half* out_row = p.out + row[i] * p.ldo;
-#pragma unroll
-                for (int j = 0; j < HN / 8; ++j) {
-                    float v[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
-                    float g[2] = {acc[4 * (j + HN / 8) + 2 * i], acc[4 * (j + HN / 8) + 2 * i + 1]};
-                    float2 bv = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
-                    if (p.ln_stats) {
-                        const float2 cv = ld_f2(p.ln_csum + a_base + 8 * j), cg = ld_f2(p.ln_csum + a_base + HN + 8 * j);
-                        bv = ld_f2(p.ln_bias + a_base + 8 * j);
-                        bg = ld_f2(p.ln_bias + a_base + HN + 8 * j);
-                        v[0] = ln_rstd[i] * (v[0] - ln_mu[i] * cv.x);
-                        v[1] = ln_rstd[i] * (v[1] - ln_mu[i] * cv.y);
-                        g[0] = ln_rstd[i] * (g[0] - ln_mu[i] * cg.x);
-                        g[1] = ln_rstd[i] * (g[1] - ln_mu[i] * cg.y);
-                    } else if (p.bias) {
-                        bv = ld_h2(p.bias + a_base + 8 * j);
-                        bg = ld_h2(p.bias + a_base + HN + 8 * j);
-                    }
-                    // the reference rounds proj output, gelu(gate) and the product to fp16
-                    const float r0 = lb_round_h(v[0] + bv.x) * lb_round_h(gelu_erf(lb_round_h(g[0] + bg.x)));
-                    const float r1 = lb_round_h(v[1] + bv.y) * lb_round_h(gelu_erf(lb_round_h(g[1] + bg.y)));
-                    *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
-                }
-            }
+        for (int hh = 0; hh < kHalves; ++hh) {
+            if (p.mode == 0) epilogue_linear<BN>(p, acc[hh], er[hh], n_tile, quad);
+            else if constexpr (BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
         }
     }
 }
@@ -382,11 +524,11 @@ template <int BN> int launch_bn(const GemmPlan& plan, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
         LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<BN>::smem_bytes(Cfg<BN>::deep)));
+                                           Cfg<BN>::smem_bytes));
         attr_set = true;
     }
     LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
-                                (size_t)Cfg<BN>::smem_bytes(plan.p.stages), st, plan.p));
+                                (size_t)Cfg<BN>::smem_bytes, st, plan.p));
     return 0;
 }
 
@@ -429,16 +571,23 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     // --- N tiling
     int bn;
     if ((d.mode & 0xff) == 1) {
-        bn = (d.mode & LB_GEMM_GEGLU256) ? 256 : 128;      // the weight rows are interleaved per N tile by the caller
+        bn = kGegluBN;      // the weight rows are interleaved per 128-row N tile by the caller
         LB_REQUIRE(d.N % bn == 0, "gemm: GEGLU needs N %% %d == 0 (got %d)", bn, d.N);
-    } else if (d.N % 256 == 0 && (int64_t)p.tiles_m * (d.N / 256) >= 2 * ctx->sm_count) bn = 256;
-    else if (d.N % 160 == 0) bn = 160;
+    } else if (d.N % 256 == 0 && d.N >= 512 && (int64_t)(d.taps * d.a0_c + (d.a1 ? d.a1_c : 0)) >= 4096 &&
+               (int64_t)p.tiles_m * (d.N / 256) >= 2 * ctx->sm_count) {
+        // Long-K, many-tile convolutions (VAE decoder at 512 channels, the 64^2 upsample conv at batch 4): the
+        // epilogue is a small share of a tile, and N = 256 wgmmas read less shared memory per FLOP than the
+        // ping-pong tiles, so the cooperative 128 x 256 tile is faster there (measured per shape on H100).
+        bn = 256;
+    } else if (d.N % 160 == 0) bn = 160;
     else if (d.N % 128 == 0) bn = 128;
     else if (d.N <= 64) bn = 64;
     else bn = 128;
     plan->bn = bn;
     p.tiles_n = (int)lb_ceil_div(d.N, bn);
     p.N = d.N;
+    LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU)) == 0, "gemm: unknown mode flags 0x%x", d.mode);
+    LB_REQUIRE((d.mode & 0xff) <= 1, "gemm: unknown epilogue mode %d", d.mode & 0xff);
     p.mode = d.mode & 0xff;
     p.static_w = (d.mode & LB_GEMM_STATIC_W) ? 1 : 0;
     // --- K segments
@@ -500,8 +649,6 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
         const int tiles = p.tiles_m * p.tiles_n;
         plan->grid = tiles < ctx->sm_count ? tiles : ctx->sm_count;
     }
-    // ring depth: as many stages as 227 KB of shared memory hold (one CTA per SM)
-    p.stages = (bn <= 64) ? 8 : (bn <= 128) ? 7 : (bn <= 160) ? 6 : 4;
     return 0;
 }
 

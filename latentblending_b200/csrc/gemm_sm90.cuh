@@ -34,7 +34,6 @@ struct alignas(64) GemmParams {
     int tiles_x, tiles_y, tiles_m, tiles_n;
     int N;
     int mode;
-    int stages;    // depth of the smem ring for this launch
     int static_w;  // weights may be fetched before griddepcontrol.wait (LB_GEMM_STATIC_W)
     __half* out; long long ldo;
     const __half* bias;
@@ -51,7 +50,7 @@ struct alignas(64) GemmParams {
 
 struct GemmPlan {
     GemmParams p;
-    int bn;        // N tile: 64 / 128 / 160 / 256
+    int bn;        // N tile: 64 / 128 / 160
     int grid;
 };
 

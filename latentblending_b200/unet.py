@@ -27,7 +27,7 @@ from typing import Tuple
 import torch
 
 from . import _cabi
-from ._cabi import (GEMM_GEGLU256, GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_CONV_OUT, OP_EMBED_INPUTS, OP_GEMM,
+from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_CONV_OUT, OP_EMBED_INPUTS, OP_GEMM,
                     OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
                     OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS, OP_UPSAMPLE2X, Op, check, ctx,
                     stream_ptr)
@@ -309,11 +309,10 @@ def _geglu_perm(inner, device, half=64):
 class PackedUNet:
     """fp16 device copies of the UNet parameters in the layouts the kernels consume."""
 
-    def __init__(self, cfg: UNetConfig, state_dict, device, fold_ln=True, geglu_tile=128):
+    def __init__(self, cfg: UNetConfig, state_dict, device, fold_ln=True):
         self.cfg = cfg
         self.device = torch.device(device)
         self.fold_ln = fold_ln
-        self.geglu_tile = geglu_tile          # N tile of the GEGLU FF-in GEMM: its weight rows are interleaved per tile
         sd = state_dict
         dev = self.device
 
@@ -377,7 +376,7 @@ class PackedUNet:
                 W[t + ".attn2.kv.w"] = torch.cat([g(t + ".attn2.to_k.weight"), g(t + ".attn2.to_v.weight")], 0).contiguous()
                 W[t + ".attn2.out.w"], W[t + ".attn2.out.b"] = g(t + ".attn2.to_out.0.weight"), g(t + ".attn2.to_out.0.bias")
                 pw, pb = g(t + ".ff.net.0.proj.weight"), g(t + ".ff.net.0.proj.bias")
-                perm = _geglu_perm(pw.shape[0] // 2, dev, half=geglu_tile // 2)
+                perm = _geglu_perm(pw.shape[0] // 2, dev)     # per 128-column N tile of the GEGLU GEMM
                 if fold_ln:
                     # LayerNorm folded into the consuming GEMM (include/lb200.h): w' = w*gamma, csum = rowsum(w'),
                     # lnb = w beta + bias
@@ -416,14 +415,7 @@ class UNetB200:
         if fold_ln is None:
             fold_ln = os.environ.get("LB_LN_FOLD") is not None
         self.fold_ln = fold_ln
-        # GEGLU N tile: 256 (N = 256 MMAs re-read the activation tile half as often) when every FF width allows it;
-        # LB_GEGLU_TILE=128 restores 128.
-        tile = int(os.environ.get("LB_GEGLU_TILE", "256"))
-        widths = [c for c, d in zip(cfg.block_out_channels, cfg.transformer_layers) if d]
-        if tile == 256 and any((8 * c) % 256 for c in widths):
-            tile = 128
-        self.geglu_tile = tile
-        self.packed = PackedUNet(cfg, state_dict, self.device, fold_ln=fold_ln, geglu_tile=tile)
+        self.packed = PackedUNet(cfg, state_dict, self.device, fold_ln=fold_ln)
         self._plans = {}
 
     # -- public -----------------------------------------------------------------------------
@@ -554,7 +546,7 @@ class _Lowering:
         kv_cache = {}
 
         fold = net.fold_ln
-        geglu_mode = 1 | (GEMM_GEGLU256 if net.geglu_tile == 256 else 0)
+        geglu_mode = 1
         f32 = dict(dtype=torch.float32, device=dev)
 
         def transformer(aname, x, C, level, out):

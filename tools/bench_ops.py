@@ -46,7 +46,7 @@ def main():
             print(json.dumps(dict(op="attention", B=B, heads=heads, S=S, Skv=Skv, us=t * 1e6, tflops=fl / t / 1e12)))
     if "gemm" in which:
         shapes = [("to_out/q/proj", 2048, 1280, 1280, 1), ("ff_out", 2048, 1280, 5120, 1), ("qkv", 2048, 3840, 1280, 1),
-                  ("ff_in_geglu", 2048, 10240, 1280, 1), ("ff_in_geglu256", 2048, 10240, 1280, 1), ("qkv64", 8192, 1920, 640, 1), ("ff_out64", 8192, 640, 2560, 1),
+                  ("ff_in_geglu", 2048, 10240, 1280, 1), ("qkv64", 8192, 1920, 640, 1), ("ff_out64", 8192, 640, 2560, 1),
                   ("conv320", 32768, 320, 320, 9), ("conv640", 8192, 640, 640, 9), ("conv1280", 2048, 1280, 1280, 9),
                   ("conv_up", 32768, 640, 640, 9), ("conv2560", 2048, 1280, 2560, 9), ("M4096", 4096, 1280, 1280, 1)]
         for name, M, N, K, taps in shapes:
@@ -60,7 +60,7 @@ def main():
             else:
                 a = torch.randn(M, K, device="cuda").half()
                 w = (torch.randn(N, K, device="cuda") * 0.02).half()
-                mode = (1 | (0x400 if "256" in name else 0)) if "geglu" in name else 0
+                mode = 1 if "geglu" in name else 0
                 out = torch.empty(M, N // 2 if mode else N, device="cuda", dtype=torch.float16)
                 f = lambda: ops.gemm(a, w, N, 1, 1, M, out=out, mode=mode, static_w=True)
                 fl = 2 * M * N * K
