@@ -110,7 +110,12 @@ int lb_cfg_euler_step(lb_ctx* ctx, const void* latents_dev, const void* eps_dev,
  * by lb_gemm_stats_parts).  Fixed summation order: results do not depend on the batch size.
  * Replaces the cuBLAS / cuDNN calls under pipe.unet(...)
  * (diffusers_holder.py:336-344).  Constraints: a0_c, a1_c multiples of 64;
- * N multiple of 8; W >= 128 or W, (H) powers of two; 16-byte aligned bases.
+ * N multiple of 8; 16-byte aligned bases; any B, H, W with B*H*W < 2^31.
+ * M tiling: 128-row tiles are either a box of pixels (tw x th x tb: 128 x 1 x 1 when W >= 128; needs W, and H when
+ * H*W < 128, to be powers of two below that) or pixel runs (tile m = rows [128m, 128m+128) of the flattened NHWC
+ * order, loaded with TMA im2col; any W and H).  By default the one with fewer tiles is used and a tie keeps the box;
+ * LB_GEMM_TILE_BOX / LB_GEMM_TILE_RUNS force one (forcing the box on a shape it cannot tile is an error).  Both give
+ * bit-identical results.
  */
 typedef struct lb_gemm_desc {
     const void* a0; int64_t a0_ld; int32_t a0_c;
@@ -123,7 +128,8 @@ typedef struct lb_gemm_desc {
     const void* bias2; int64_t bias2_ld;
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
-    int32_t mode;     /* low byte: 0 = linear epilogue, 1 = GEGLU; flags: LB_GEMM_STATIC_W, LB_GEMM_RELU */
+    int32_t mode;     /* low byte: 0 = linear epilogue, 1 = GEGLU; flags: LB_GEMM_STATIC_W, LB_GEMM_RELU,
+                         LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS */
     const void* ln_stats; int32_t ln_parts;      /* float2 [M][ln_parts] or NULL */
     const void* ln_csum; const void* ln_bias;    /* float [N] each */
     float ln_eps;
@@ -134,6 +140,10 @@ typedef struct lb_gemm_desc {
 #define LB_GEMM_STATIC_W 0x100
 /* mode flag (linear epilogue): out = max(out, 0) -- the AlexNet convolutions of the LPIPS metric */
 #define LB_GEMM_RELU 0x200
+/* mode flags: force the pixel-box (LB_GEMM_TILE_BOX) or the pixel-run (LB_GEMM_TILE_RUNS) M tiling instead of the
+ * automatic choice; at most one of them */
+#define LB_GEMM_TILE_BOX 0x400
+#define LB_GEMM_TILE_RUNS 0x800
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
 /* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
  * that holds a row of the wgmma accumulator); < 0 on error */

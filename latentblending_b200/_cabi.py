@@ -95,6 +95,8 @@ class Op(ctypes.Structure):
 
 GEMM_STATIC_W = 0x100     # lb_gemm_desc.mode flag (include/lb200.h: LB_GEMM_STATIC_W)
 GEMM_RELU = 0x200         # LB_GEMM_RELU
+GEMM_TILE_BOX = 0x400     # LB_GEMM_TILE_BOX: force the pixel-box M tiling
+GEMM_TILE_RUNS = 0x800    # LB_GEMM_TILE_RUNS: force the pixel-run M tiling
 (OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN, OP_CONV_OUT,
  OP_UPSAMPLE2X, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
  OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = range(1, 18)

@@ -38,6 +38,7 @@ extern "C" int lb_ctx_create(int device, lb_ctx** out) {
     c->sm_count = prop.multiProcessorCount;
     c->smem_optin = (int)prop.sharedMemPerBlockOptin;
     c->tmap_encode = nullptr;
+    c->tmap_encode_im2col = nullptr;
     c->err_flag_dev = nullptr;
     LB_CHECK_CUDA(cudaSetDevice(device));
     LB_CHECK_CUDA(cudaMalloc(&c->err_flag_dev, sizeof(int)));

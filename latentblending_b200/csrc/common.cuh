@@ -14,6 +14,7 @@ struct lb_ctx {
     int sm_count;
     int smem_optin;       // max dynamic smem per block (bytes)
     void* tmap_encode;    // cuTensorMapEncodeTiled, resolved lazily through the runtime
+    void* tmap_encode_im2col;   // cuTensorMapEncodeIm2col, likewise
     int* err_flag_dev;    // protocol-error code written by a kernel before it traps
 };
 

@@ -10,6 +10,14 @@
 // by (dy,dx) with hardware zero fill at the borders -- no im2col buffer), and
 // the resnet shortcut folded in as an extra K-segment from a second tensor.
 //
+// Two M tilings (gemm_plan_build picks the one with fewer tiles; a tie keeps the box):
+//   box  : a 128-row tile is a tw x th x tb box of pixels (128 x 1 x 1 when W >= 128; W and, if H*W < 128, H powers
+//          of two otherwise), one tiled TMA load per k-block;
+//   runs : tile m is rows [128 m, 128 m + 128) of the flattened pixel order, any W and H; one TMA im2col load per
+//          k-block fetches the 128 pixels (across row and image boundaries) shifted by the filter tap.
+// Both fill the same 128 x 128 B swizzled A tile, and every output element is the same k-ordered dot product, so
+// the two give bit-identical results wherever both apply.
+//
 // Structure (one CTA per SM, persistent over 128 x BN output tiles, 384 threads = three warpgroups):
 //   warpgroup 0   : TMA producer -- one warp issues cp.async.bulk.tensor 4D (A) / 2D (W) into a STAGES-deep
 //                   128B-swizzled smem ring, mbarrier full/empty pairs, in the CTA's tile order; the warpgroup gives
@@ -262,7 +270,8 @@ __device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float 
     }
 }
 
-template <int BN>
+// kRuns: pixel-run M tiles (p.runs = 1); a separate instantiation, so the pixel-box kernels stay as they were
+template <int BN, bool kRuns>
 __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
     using C = Cfg<BN>;
     constexpr int nst = C::stages;
@@ -325,9 +334,20 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
         uint32_t phase = 0;
         for (int tile = tile0; tile < num_tiles; tile += tile_step) {
             const int m_tile = tile % m_groups, n_tile = tile / m_groups;
-            const int x0 = (m_tile % p.tiles_x) * p.tw;
-            const int y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.th;
-            const int b0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.tb;
+            // box: the tile's corner pixel (x0, y0, b0); runs: the pixel-box coordinate of the run's first pixel,
+            // whose box starts one pixel up and left of the image (see encode_act_map_runs)
+            int x0, y0, b0;
+            if constexpr (kRuns) {
+                const int row0 = m_tile * kBM;
+                b0 = row0 / p.HW;
+                const int rem = row0 - b0 * p.HW;
+                y0 = rem / p.W - 1;
+                x0 = rem % p.W - 1;
+            } else {
+                x0 = (m_tile % p.tiles_x) * p.tw;
+                y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.th;
+                b0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.tb;
+            }
             int kb_global = 0;
             for (int s = 0; s < p.num_segs; ++s) {
                 const CUtensorMap* ma = &p.tmA[p.seg_map[s]];
@@ -335,12 +355,21 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
                 for (int kb = 0; kb < p.seg_kb[s]; ++kb, ++kb_global) {
                     mbar_wait(&empty[stage], phase ^ 1, p.err_flag, 1);
                     if (elect_one()) {
+                        // filter tap (dy, dx) in {-1, 0, 1}^2: a box shifted by (dx, dy), or a run read at im2col
+                        // offset (dx + 1, dy + 1)
+                        const auto load_a = [&]() {
+                            if constexpr (kRuns)
+                                tma_load_4d_im2col(smem_a + stage * kABytes, ma, &full[stage], kb * kBK, x0, y0, b0,
+                                                   (uint16_t)(dx + 1), (uint16_t)(dy + 1));
+                            else
+                                tma_load_4d(smem_a + stage * kABytes, ma, &full[stage], kb * kBK, x0 + dx, y0 + dy, b0);
+                        };
                         if (tile == tile0 && kb_global < early_kb) {
                             // expect_tx and the weight tile were issued before griddepcontrol.wait
-                            tma_load_4d(smem_a + stage * kABytes, ma, &full[stage], kb * kBK, x0 + dx, y0 + dy, b0);
+                            load_a();
                         } else {
                             mbar_expect_tx(&full[stage], C::stage_bytes);
-                            tma_load_4d(smem_a + stage * kABytes, ma, &full[stage], kb * kBK, x0 + dx, y0 + dy, b0);
+                            load_a();
                             tma_load_2d(smem_b + stage * C::b_bytes, &p.tmB, &full[stage], kb_global * kBK, n_tile * BN);
                         }
                     }
@@ -372,10 +401,17 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
         EpiRow er[kHalves][2];
         const auto row_of = [&](int hh, int i) {
             const int rr = half_of(hh) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+            EpiRow& e = er[hh][i];
+            if constexpr (kRuns) {     // a run may span images: each row takes its own image's bias2 row
+                const int row = m_tile * kBM + rr;
+                e.ok = row < p.M;
+                e.row = (unsigned)row;      // row >= 0: zero extension leaves no high word to keep live
+                e.bidx = row / p.HW;
+                return;
+            }
             const int x = (m_tile % p.tiles_x) * p.tw + rr % p.tw;
             const int y = ((m_tile / p.tiles_x) % p.tiles_y) * p.th + (rr / p.tw) % p.th;
             const int b = (m_tile / (p.tiles_x * p.tiles_y)) * p.tb + rr / (p.tw * p.th);
-            EpiRow& e = er[hh][i];
             e.ok = (x < p.W) && (y < p.H) && (b < p.B);
             e.row = ((long long)b * p.H + y) * p.W + x;
             e.bidx = b;
@@ -446,18 +482,25 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
         for (int hh = 0; hh < kHalves; ++hh) fence_regs(acc[hh]);
         if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty[prev_stage]);
-#pragma unroll
-        for (int hh = 0; hh < kHalves; ++hh)
+        // Pixel runs form a half's rows just before its epilogue, which keeps them out of the other half's register
+        // live range (the BN = 160 run kernel spills otherwise); the box kernels form all rows first.
+        const auto rows_of_half = [&](int hh) {
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 row_of(hh, i);
                 er[hh][i].ln_mu = ln_mu[hh][i];
                 er[hh][i].ln_rstd = ln_rstd[hh][i];
             }
+        };
+        if constexpr (!kRuns) {
+#pragma unroll
+            for (int hh = 0; hh < kHalves; ++hh) rows_of_half(hh);
+        }
 
         // ---- epilogue from registers (in ping-pong, overlapping the other warpgroup's main loop)
 #pragma unroll
         for (int hh = 0; hh < kHalves; ++hh) {
+            if constexpr (kRuns) rows_of_half(hh);
             if (p.mode == 0) epilogue_linear<BN>(p, acc[hh], er[hh], n_tile, quad);
             else if constexpr (BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
         }
@@ -501,6 +544,45 @@ int encode_act_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, in
     return 0;
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+
+int get_encode_im2col(lb_ctx* ctx, EncodeIm2colFn* fn) {
+    if (!ctx->tmap_encode_im2col) {
+        void* f = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        LB_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &f, cudaEnableDefault, &qres));
+        LB_REQUIRE(f != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeIm2col not available");
+        ctx->tmap_encode_im2col = f;
+    }
+    *fn = reinterpret_cast<EncodeIm2colFn>(ctx->tmap_encode_im2col);
+    return 0;
+}
+
+// 4-D NHWC activation map for pixel-run tiles: dims (C, W, H, B), im2col mode, 128 pixels x 64 channels per load,
+// 128B swizzle, zero OOB fill.  The pixel bounding box runs from (-1, -1) to (W - 2, H - 2) in (x, y): W x H positions
+// per image, so a run of 128 consecutive box positions is 128 consecutive output pixels.  The position of output pixel
+// (x, y) is (x - 1, y - 1); with im2col offset (dx + 1, dy + 1) it reads input pixel (x + dx, y + dy), the 3x3 tap
+// (dy, dx) at padding 1 (a 1x1 segment uses offset (1, 1)).
+int encode_act_map_runs(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int C, int W, int H, int B) {
+    EncodeIm2colFn enc;
+    if (int e = get_encode_im2col(ctx, &enc)) return e;
+    LB_REQUIRE(lb_aligned16(base), "activation base must be 16-byte aligned");
+    LB_REQUIRE(ld % 8 == 0 && ld >= C, "activation row stride must be a multiple of 8 elements and >= C");
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)ld * 2 * W, (cuuint64_t)ld * 2 * W * H};
+    const int lower[2] = {-1, -1}, upper[2] = {-1, -1};     // (W, H)
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, lower, upper,
+                     (cuuint32_t)kBK, (cuuint32_t)kBM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    LB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col(activation C=%d W=%d H=%d B=%d ld=%lld) failed: %d", C, W, H,
+               B, (long long)ld, (int)r);
+    return 0;
+}
+
 int encode_weight_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int64_t K, int N, int bn) {
     EncodeTiledFn enc;
     if (int e = get_encode(ctx, &enc)) return e;
@@ -520,16 +602,37 @@ int encode_weight_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld,
 
 bool is_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
-template <int BN> int launch_bn(const GemmPlan& plan, cudaStream_t st) {
+// The pixel box of 128 rows for this shape; nullptr, or why the box cannot tile it.
+const char* box_tiling(const GemmDesc& d, int* tw, int* th, int* tb) {
+    if (d.W >= kBM || (d.H == 1 && d.B == 1)) {   // rows of a plain matrix: ragged tail is zero-filled by TMA
+        *tw = kBM; *th = 1; *tb = 1;
+        return nullptr;
+    }
+    if (!is_pow2(d.W)) return "W < 128 must be a power of two";
+    *tw = d.W;
+    *th = kBM / d.W;
+    if (*th > d.H) {
+        if (!is_pow2(d.H)) return "H must be a power of two when H*W < 128";
+        *th = d.H;
+    }
+    *tb = kBM / (*tw * *th);
+    return nullptr;
+}
+
+template <int BN, bool kRuns> int launch_tiled(const GemmPlan& plan, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, kRuns>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            Cfg<BN>::smem_bytes));
         attr_set = true;
     }
-    LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
+    LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN, kRuns>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
                                 (size_t)Cfg<BN>::smem_bytes, st, plan.p));
     return 0;
+}
+
+template <int BN> int launch_bn(const GemmPlan& plan, cudaStream_t st) {
+    return plan.p.runs ? launch_tiled<BN, true>(plan, st) : launch_tiled<BN, false>(plan, st);
 }
 
 }  // namespace
@@ -548,26 +651,42 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     LB_REQUIRE(!d.bias2 || (lb_aligned16(d.bias2) && d.bias2_ld % 8 == 0), "gemm: bias2 alignment");
     GemmParams& p = plan->p;
     memset(&p, 0, sizeof(p));
-    // --- M tiling: a 128-row tile is a (tw x th x tb) box of pixels
-    int tw, th, tb;
-    if (d.W >= kBM || (d.H == 1 && d.B == 1)) {   // rows of a plain matrix: ragged tail is zero-filled by TMA
-        tw = kBM; th = 1; tb = 1;
+    LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS)) == 0,
+               "gemm: unknown mode flags 0x%x", d.mode);
+    const int force = d.mode & (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS);
+    LB_REQUIRE(force != (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS), "gemm: LB_GEMM_TILE_BOX and LB_GEMM_TILE_RUNS exclude "
+               "each other");
+    // --- M tiling: the pixel box or pixel runs, whichever needs fewer 128-row tiles (a tie keeps the box)
+    const int64_t M = (int64_t)d.B * d.H * d.W;
+    const int64_t run_tiles = lb_ceil_div(M, kBM);
+    int tw = kBM, th = 1, tb = 1;
+    const char* box_err = box_tiling(d, &tw, &th, &tb);
+    int64_t box_tiles = -1;
+    if (!box_err) box_tiles = lb_ceil_div(d.W, tw) * lb_ceil_div(d.H, th) * lb_ceil_div(d.B, tb);
+    bool runs;
+    if (force == LB_GEMM_TILE_BOX) {
+        LB_REQUIRE(!box_err, "gemm: the pixel box cannot tile B=%d H=%d W=%d: %s", d.B, d.H, d.W, box_err);
+        runs = false;
+    } else if (force == LB_GEMM_TILE_RUNS) {
+        runs = true;
     } else {
-        LB_REQUIRE(is_pow2(d.W), "gemm: W (%d) < 128 must be a power of two", d.W);
-        tw = d.W;
-        th = kBM / tw;
-        if (th > d.H) {
-            LB_REQUIRE(is_pow2(d.H), "gemm: H (%d) must be a power of two when H*W < 128", d.H);
-            th = d.H;
-        }
-        tb = kBM / (tw * th);
+        runs = box_err != nullptr || run_tiles < box_tiles;
     }
-    p.tw = tw; p.th = th; p.tb = tb;
     p.W = d.W; p.H = d.H; p.B = d.B;
-    p.tiles_x = (int)lb_ceil_div(d.W, tw);
-    p.tiles_y = (int)lb_ceil_div(d.H, th);
-    const int tiles_b = (int)lb_ceil_div(d.B, tb);
-    p.tiles_m = p.tiles_x * p.tiles_y * tiles_b;
+    p.runs = runs ? 1 : 0;
+    if (runs) {
+        LB_REQUIRE(M <= 0x7fffffff, "gemm: pixel runs need B*H*W < 2^31 (got %lld)", (long long)M);
+        p.M = (int)M;
+        p.HW = d.H * d.W;
+        p.tw = kBM; p.th = 1; p.tb = 1;
+        p.tiles_x = p.tiles_y = 1;
+        p.tiles_m = (int)run_tiles;
+    } else {
+        p.tw = tw; p.th = th; p.tb = tb;
+        p.tiles_x = (int)lb_ceil_div(d.W, tw);
+        p.tiles_y = (int)lb_ceil_div(d.H, th);
+        p.tiles_m = (int)box_tiles;
+    }
     // --- N tiling
     int bn;
     if ((d.mode & 0xff) == 1) {
@@ -586,7 +705,6 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     plan->bn = bn;
     p.tiles_n = (int)lb_ceil_div(d.N, bn);
     p.N = d.N;
-    LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU)) == 0, "gemm: unknown mode flags 0x%x", d.mode);
     LB_REQUIRE((d.mode & 0xff) <= 1, "gemm: unknown epilogue mode %d", d.mode & 0xff);
     p.mode = d.mode & 0xff;
     p.static_w = (d.mode & LB_GEMM_STATIC_W) ? 1 : 0;
@@ -609,9 +727,13 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     p.num_segs = ns;
     p.total_kb = total;
     const int64_t Ktot = (int64_t)total * kBK;
-    if (int e = encode_act_map(ctx, &p.tmA[0], d.a0, d.a0_ld, d.a0_c, d.W, d.H, d.B, tw, th, tb)) return e;
+    const auto encode_a = [&](CUtensorMap* m, const void* base, int64_t ld, int c) {
+        return runs ? encode_act_map_runs(ctx, m, base, ld, c, d.W, d.H, d.B)
+                    : encode_act_map(ctx, m, base, ld, c, d.W, d.H, d.B, tw, th, tb);
+    };
+    if (int e = encode_a(&p.tmA[0], d.a0, d.a0_ld, d.a0_c)) return e;
     if (d.a1) {
-        if (int e = encode_act_map(ctx, &p.tmA[1], d.a1, d.a1_ld, d.a1_c, d.W, d.H, d.B, tw, th, tb)) return e;
+        if (int e = encode_a(&p.tmA[1], d.a1, d.a1_ld, d.a1_c)) return e;
     } else {
         p.tmA[1] = p.tmA[0];
     }

@@ -15,6 +15,7 @@ struct GemmDesc {
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
     int32_t mode;   // low byte: 0 linear epilogue, 1 GEGLU (N accumulators -> N/2 outputs); | LB_GEMM_STATIC_W | LB_GEMM_RELU
+                    // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS
     // LayerNorm folded into this GEMM (see include/lb200.h)
     const void* ln_stats; int32_t ln_parts;
     const void* ln_csum; const void* ln_bias; float ln_eps;
@@ -30,7 +31,7 @@ struct alignas(64) GemmParams {
     int seg_map[kGemmMaxSegs], seg_dy[kGemmMaxSegs], seg_dx[kGemmMaxSegs], seg_kb[kGemmMaxSegs];
     int total_kb;
     int W, H, B;
-    int tw, th, tb;
+    int tw, th, tb;        // pixel-box tiling: a tile is a (tw x th x tb) box, tiles_x * tiles_y * ceil(B / tb) of them
     int tiles_x, tiles_y, tiles_m, tiles_n;
     int N;
     int mode;
@@ -46,6 +47,10 @@ struct alignas(64) GemmParams {
     const float2* ln_stats; int ln_parts; float ln_inv_k, ln_eps;
     const float* ln_csum; const float* ln_bias;
     float2* stats_out;     // [M][4*tiles_n]: (sum, sum of squares) of this launch's fp16 outputs per row and column part
+    // pixel-run tiling (runs = 1): tile m is rows [128 m, 128 m + 128) of the flattened b*H*W + y*W + x pixel order
+    // (it may span image rows and images; M = B*H*W < 2^31), loaded by TMA im2col runs
+    int runs;
+    int M, HW;
 };
 
 struct GemmPlan {

@@ -85,6 +85,17 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
         "r"(c3)
         : "memory");
 }
+// im2col mode: a run of the map's pixelsPerColumn consecutive pixels (W fastest, then H, then N, inside the map's
+// pixel bounding box) starting at box coordinate (c1, c2, c3), each pixel read at its position + (off_w, off_h),
+// channelsPerPixel channels from c0; positions outside the tensor are zero-filled.
+__device__ __forceinline__ void tma_load_4d_im2col(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                   int c2, int c3, uint16_t off_w, uint16_t off_h) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
+        "r"(c3), "h"(off_w), "h"(off_h)
+        : "memory");
+}
 
 // ---- register budget of warp-specialised kernels (per warpgroup, multiple of 8) ----------------
 template <int R> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }

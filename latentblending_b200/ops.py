@@ -113,10 +113,17 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
+_TILING = {"auto": 0, "box": _cabi.GEMM_TILE_BOX, "runs": _cabi.GEMM_TILE_RUNS}
+
+
 def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None, out=None,
-         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None):
+         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto"):
     """Tensor-core GEMM / implicit-GEMM conv (lb_gemm).  a0: NHWC activation viewed as
-    [B*H*W, >=a0_c] (row stride = a0.stride(0)); w: [N, K] packed weights."""
+    [B*H*W, >=a0_c] (row stride = a0.stride(0)); w: [N, K] packed weights.
+    ``tiling``: "auto" (the M tiling with fewer tiles), "box" (pixel boxes) or "runs" (pixel runs); all give the
+    same results."""
+    if tiling not in _TILING:
+        raise ValueError(f"tiling must be one of {sorted(_TILING)} (got {tiling!r})")
     dev = _dev(a0)
     M = B * H * W
     a0_c = a0.shape[-1] if a0_c is None else a0_c
@@ -135,7 +142,7 @@ def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bi
     if res is not None:
         d.res, d.res_ld = _p(res), res.stride(-2)
     d.out, d.out_ld = _p(out), out.stride(-2)
-    d.mode = mode | (_cabi.GEMM_STATIC_W if static_w else 0) | (_cabi.GEMM_RELU if relu else 0)
+    d.mode = mode | (_cabi.GEMM_STATIC_W if static_w else 0) | (_cabi.GEMM_RELU if relu else 0) | _TILING[tiling]
     if ln is not None:
         d.ln_stats, d.ln_parts = _p(ln["stats"]), ln["stats"].shape[1]
         d.ln_csum, d.ln_bias, d.ln_eps = _p(ln["csum"]), _p(ln["bias"]), ln["eps"]

@@ -160,11 +160,14 @@ class _VAELowering:
         P.groupnorm(x2, B, S, C0, groups, Wt["attn.norm.g"], Wt["attn.norm.b"], 1e-6, 0, hn, self.ws)
         qk = torch.empty(S, 2 * C0, **f16)
         P.gemm(hn, Wt["attn.qk.w"], 2 * C0, 1, 1, S, qk, bias=Wt["attn.qk.b"])
-        vT = torch.empty(C0, S, **f16)
-        P.gemm(Wt["attn.v.w"], hn, S, 1, 1, C0, vT, static_w=False)                       # V^T = Wv hn^T
-        scores = torch.empty(S, S, **f16)
-        P.gemm(qk[:, :C0], qk[:, C0:], S, 1, 1, S, scores, static_w=False)               # (scaled q) k^T
-        P.softmax_rows(scores, scores)
+        # P V contracts over the S keys, and the GEMM's K must be a multiple of 64: P and V^T get Sp >= S columns, the
+        # extra ones zero (never written), which adds exact zeros to every dot product
+        Sp = -(-S // 64) * 64
+        vT = torch.zeros(C0, Sp, **f16)
+        P.gemm(Wt["attn.v.w"], hn, S, 1, 1, C0, vT[:, :S], static_w=False)               # V^T = Wv hn^T
+        scores = torch.zeros(S, Sp, **f16)
+        P.gemm(qk[:, :C0], qk[:, C0:], S, 1, 1, S, scores[:, :S], static_w=False)        # (scaled q) k^T
+        P.softmax_rows(scores[:, :S], scores[:, :S])
         att = sc("h1", S, C0)
         P.gemm(scores, vT, C0, 1, 1, S, att, static_w=False)                              # P V
         x3 = torch.empty(S, C0, **f16)
