@@ -192,7 +192,15 @@ int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
  *   act: 0 none, 1 SiLU.
  * lb_conv_in / lb_conv_out: the 4->C0 and C0->4 3x3 convolutions at the NCHW
  *   latent boundary.  lb_upsample2x: nearest 2x (Upsample2D).  lb_im2col_s2: patch
- *   matrix of the stride-2 Downsample2D convs (then lb_gemm).
+ *   matrix of the stride-2 Downsample2D convs (then lb_gemm); its output is
+ *   ceil(H/2) x ceil(W/2), so any H and W.
+ * lb_upsample_nearest: F.interpolate(size=(Ho, Wo), mode="nearest") of an H x W
+ *   map for Ho in {2H-1, 2H} and Wo in {2W-1, 2W} (any other size is an error):
+ *   the Upsample2D of an up block whose skip level has an odd side (diffusers'
+ *   forward_upsample_size, latent sides not divisible by 2^(levels-1)).  Output
+ *   pixel (yo, xo) is input pixel (yo >> 1, xo >> 1), i.e. nearest 2x cropped to
+ *   Ho x Wo.  lb_upsample2x is the Ho = 2H, Wo = 2W case.  C and both row strides
+ *   multiples of 8.
  */
 int lb_embed_inputs(lb_ctx* ctx, float t, const void* text_embeds, const void* time_ids, int B,
                     int dim_t, int pooled, int dim_a, void* temb_in, void* add_in, void* stream);
@@ -205,12 +213,15 @@ int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, i
                 const void* bias, int Cout, void* out_nchw, void* stream);
 int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
                   void* stream);
+int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
+                        int Ho, int Wo, void* stream);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
 
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
  * lb_latent_prep: post_quant_conv(latents / scaling_factor) as a per-pixel CxC fp32 matrix (scale folded in).
  * lb_softmax_rows: row softmax of an fp16 matrix (the VAE mid-block single-head attention, head dim 512,
- *   runs as lb_gemm(Q,K) -> lb_softmax_rows -> lb_gemm(P,V^T)).
+ *   runs as lb_gemm(Q,K) -> lb_softmax_rows -> lb_gemm(P,V^T)).  Any cols; row strides multiples of 8, bases
+ *   16-byte aligned.
  * lb_postprocess_u8: (x/2+0.5).clamp(0,1)*255 -> uint8 NHWC (VaeImageProcessor.postprocess).  nonfinite_count_dev
  *   (optional, device int) is incremented by the number of NaN/Inf pixels: the decoder runs in fp16 where the reference
  *   upcasts the stock SDXL VAE to fp32 because it "overflows in float16" (diffusers_holder.py:128-133); an overflow
@@ -284,7 +295,8 @@ typedef struct lb_op {
                  const void* addend; int64_t ldadd; int32_t act_in, act_out; void* out; int64_t ldo; int32_t N; } lin;
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
                  int32_t Cout; void* out; int64_t ld_out; } conv;
-        struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; } resample;
+        /* UPSAMPLE2X: output Ho x Wo (0 = 2H / 2W; see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
+        struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; int32_t Ho, Wo; } resample;
         /* LATENT_PREP: x,w,bias,out,B,C,n=h*w; SOFTMAX_ROWS: x,ld_x,out,ld_out,n=rows,C=cols;
          * POSTPROCESS_U8: x,out,B,C,n=h*w, w = optional device int counter of non-finite pixels;
          * NHWC_TO_NCHW: x,ld_x,out,B,C,n=h*w */

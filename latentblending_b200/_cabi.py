@@ -70,7 +70,7 @@ class _ConvOp(ctypes.Structure):
 
 class _ResampleOp(ctypes.Structure):
     _fields_ = [("x", c_void_p), ("ld_x", c_int64), ("B", c_int32), ("H", c_int32), ("W", c_int32), ("C", c_int32),
-                ("out", c_void_p), ("ld_out", c_int64)]
+                ("out", c_void_p), ("ld_out", c_int64), ("Ho", c_int32), ("Wo", c_int32)]   # 0 = 2H / 2W
 
 
 class _AuxOp(ctypes.Structure):
@@ -141,6 +141,8 @@ SIGNATURES = {
     "lb_conv_out": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                             c_void_p, c_void_p]),
     "lb_upsample2x": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
+                                    c_int, c_void_p]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "lb_latent_prep": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lb_softmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p]),

@@ -3,7 +3,7 @@
 //       (time_embedding, add_embedding, all resnet time_emb_proj in one batched launch)
 //   K2  conv_in  (4 -> C0, 3x3, NCHW latent in, NHWC out)
 //       conv_out (C0 -> 4, 3x3, NHWC in, NCHW eps out)
-//       nearest-2x upsample, stride-2 im2col (the two Downsample2D convs then run as plain GEMMs)
+//       nearest upsample (2x, or 2x cropped by one row / column), stride-2 im2col (the two Downsample2D convs then run as plain GEMMs)
 // Replace pieces of pipe.unet(...) (call site latentblending/diffusers_holder.py:336-344;
 // diffusers 0.25.0 embeddings.py / resnet.py / unet_2d_condition.py).
 #include "common.cuh"
@@ -215,18 +215,21 @@ conv_out_kernel(const __half* __restrict__ x, long long ld, int B, int Cin, int 
     }
 }
 
-// ---- nearest 2x upsample, NHWC ------------------------------------------------------------------
+// ---- nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}), NHWC ------------------------------------
+// Nearest 2x cropped to Ho x Wo: output (yo, xo) reads input (yo >> 1, xo >> 1).  With H = ceil(Ho / 2) this is
+// exactly torch's nearest index min(floor(yo * (float)H / Ho), H - 1), so F.interpolate(size=...) needs no
+// floating-point index arithmetic here.
 __global__ void __launch_bounds__(kThreads)
-upsample2x_kernel(const __half* __restrict__ x, long long ld, int B, int H, int W, int C, __half* __restrict__ out,
-                  long long ldo) {
+upsample_nearest_kernel(const __half* __restrict__ x, long long ld, int B, int H, int W, int C, __half* __restrict__ out,
+                        long long ldo, int Ho, int Wo) {
     pdl_launch_dependents();
     pdl_wait();
     const int vecs = C >> 3;
-    const long long total = (long long)B * 2 * H * 2 * W * vecs;
+    const long long total = (long long)B * Ho * Wo * vecs;
     for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
         const int v = (int)(i % vecs);
         const long long opix = i / vecs;
-        const int xo = (int)(opix % (2 * W)), yo = (int)((opix / (2 * W)) % (2 * H)), b = (int)(opix / ((long long)4 * W * H));
+        const int xo = (int)(opix % Wo), yo = (int)((opix / Wo) % Ho), b = (int)(opix / ((long long)Wo * Ho));
         const long long ipix = ((long long)b * H + (yo >> 1)) * W + (xo >> 1);
         *reinterpret_cast<uint4*>(out + opix * ldo + v * 8) = *reinterpret_cast<const uint4*>(x + ipix * ld + v * 8);
     }
@@ -354,15 +357,23 @@ extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Ci
     return 0;
 }
 
-extern "C" int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
-                             void* stream) {
-    LB_REQUIRE(ctx && x && out, "lb_upsample2x: null argument");
-    LB_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0, "lb_upsample2x: C and strides must be multiples of 8");
-    const long long total = (long long)B * 4 * H * W * (C / 8);
-    lb_launch_pdl(upsample2x_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream), (const __half*)x, ld, B, H, W, C,
-                                                                                         (__half*)out, ldo);
+extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                                   int64_t ldo, int Ho, int Wo, void* stream) {
+    LB_REQUIRE(ctx && x && out, "lb_upsample_nearest: null argument");
+    LB_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0, "lb_upsample_nearest: C and strides must be multiples of 8");
+    LB_REQUIRE((Ho == 2 * H || Ho == 2 * H - 1) && (Wo == 2 * W || Wo == 2 * W - 1) && Ho >= 1 && Wo >= 1,
+               "lb_upsample_nearest: output %dx%d is not a nearest 2x of %dx%d (need Ho in {2H-1, 2H}, Wo in {2W-1, 2W})",
+               Ho, Wo, H, W);
+    const long long total = (long long)B * Ho * Wo * (C / 8);
+    lb_launch_pdl(upsample_nearest_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream),
+                  (const __half*)x, ld, B, H, W, C, (__half*)out, ldo, Ho, Wo);
     LB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
+                             void* stream) {
+    return lb_upsample_nearest(ctx, x, ld, B, H, W, C, out, ldo, 2 * H, 2 * W, stream);
 }
 
 extern "C" int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream) {
@@ -397,7 +408,8 @@ latent_prep_kernel(const __half* __restrict__ x, int B, int C, long long hw, con
     }
 }
 
-// row softmax (in place capable): out[r,:] = softmax(x[r,:]) over `cols` fp16 values, one CTA per row.
+// row softmax (in place capable): out[r,:] = softmax(x[r,:]) over `cols` fp16 values, one CTA per row.  Columns past
+// the last multiple of 8 (h*w keys of a VAE latent with an odd side) take a scalar tail after the 128-bit loop.
 __global__ void __launch_bounds__(kThreads)
 softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half* __restrict__ out, long long ldo) {
     pdl_launch_dependents();
@@ -418,6 +430,7 @@ softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half
             mx = fmaxf(mx, fmaxf(f.x, f.y));
         }
     }
+    for (int c = (vecs << 3) + threadIdx.x; c < cols; c += kThreads) mx = fmaxf(mx, __half2float(xr[c]));
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
@@ -439,6 +452,7 @@ softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half
             sum += __expf(f.x - mx) + __expf(f.y - mx);
         }
     }
+    for (int c = (vecs << 3) + threadIdx.x; c < cols; c += kThreads) sum += __expf(__half2float(xr[c]) - mx);
     sum = lb_warp_sum(sum);
     __syncthreads();
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
@@ -462,6 +476,8 @@ softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half
         }
         *reinterpret_cast<uint4*>(orow + v * 8) = o;
     }
+    for (int c = (vecs << 3) + threadIdx.x; c < cols; c += kThreads)
+        orow[c] = __float2half_rn(__expf(__half2float(xr[c]) - mx) * inv);
 }
 
 // NHWC rows [B*hw, ld] (first C columns) -> NCHW [B, C, hw]: the boundary of the conv_out GEMM (C = 4 eps / 3 RGB
@@ -518,8 +534,8 @@ extern "C" int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int
 extern "C" int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
                                void* stream) {
     LB_REQUIRE(ctx && x && out, "lb_softmax_rows: null argument");
-    LB_REQUIRE(cols % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0 && lb_aligned16(x) && lb_aligned16(out),
-               "lb_softmax_rows: cols / strides must be multiples of 8, bases 16B aligned");
+    LB_REQUIRE(cols >= 0 && ld % 8 == 0 && ldo % 8 == 0 && lb_aligned16(x) && lb_aligned16(out),
+               "lb_softmax_rows: strides must be multiples of 8, bases 16B aligned");
     LB_REQUIRE(rows <= 2147483647LL, "lb_softmax_rows: too many rows");
     if (rows == 0) return 0;
     lb_launch_pdl(softmax_rows_kernel, (unsigned)rows, kThreads, 0, lb_stream(stream), (const __half*)x, ld, cols, (__half*)out, ldo);

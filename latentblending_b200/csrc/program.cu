@@ -11,6 +11,9 @@
 
 #include "gemm_sm90.cuh"
 
+// the op records are an ABI: a member may grow only inside the union's existing size (set by lb_gemm_desc)
+static_assert(sizeof(((lb_op*)nullptr)->u.resample) <= sizeof(lb_gemm_desc), "lb_op.u.resample outgrew the union");
+
 struct AttnPlan;
 int attn_plan_build_opaque(lb_ctx* ctx, const lb_attn_desc& d, void** plan_out);
 int attn_plan_launch_opaque(void* plan, cudaStream_t st);
@@ -195,7 +198,8 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_UPSAMPLE2X: {
                 const auto& a = o.u.resample;
-                e = lb_upsample2x(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out, stream);
+                e = lb_upsample_nearest(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out,
+                                        a.Ho ? a.Ho : 2 * a.H, a.Wo ? a.Wo : 2 * a.W, stream);
                 break;
             }
             case LB_OP_IM2COL_S2: {

@@ -282,6 +282,17 @@ def upsample2x(x, B, H, W, C, out=None):
     return out
 
 
+def upsample_nearest(x, B, H, W, C, Ho, Wo, out=None):
+    """F.interpolate(size=(Ho, Wo), mode="nearest") of NHWC rows [B*H*W, >=C] for Ho in {2H-1, 2H}, Wo in
+    {2W-1, 2W} (lb_upsample_nearest; other sizes raise LB200Error)."""
+    dev = _dev(x)
+    if out is None:
+        out = torch.empty((B * Ho * Wo, C), dtype=torch.float16, device=x.device)
+    check(_cabi.load().lb_upsample_nearest(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), out.stride(0),
+                                           Ho, Wo, stream_ptr()), "lb_upsample_nearest")
+    return out
+
+
 def im2col_s2(x, B, H, W, C, out=None):
     dev = _dev(x)
     Ho, Wo = (H + 1) // 2, (W + 1) // 2

@@ -199,9 +199,11 @@ class Program:
         d.x, d.ld_x, d.out, d.n, d.B, d.C = _p(tmp), tmp.stride(0), _p(out_nchw), H * W, B, Cout
         self.hold(tmp, out_nchw)
 
-    def upsample2x(self, x, B, H, W, C, out):
+    def upsample2x(self, x, B, H, W, C, out, Ho=0, Wo=0):
+        """Nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}; 0 = exactly 2x)."""
         d = self._new(OP_UPSAMPLE2X).u.resample
         d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
+        d.Ho, d.Wo = Ho, Wo
         self.hold(x, out)
 
     def im2col_s2(self, x, B, H, W, C, out):
@@ -454,7 +456,6 @@ class _Lowering:
         f16 = dict(dtype=torch.float16, device=dev)
         ch = list(cfg.block_out_channels)
         L = len(ch)
-        assert H % (1 << (L - 1)) == 0 and W % (1 << (L - 1)) == 0, "latent size must be divisible by 2^(levels-1)"
         T = cfg.time_embed_dim
         groups = cfg.norm_num_groups
         if x_in is not None:
@@ -498,7 +499,10 @@ class _Lowering:
         P.linear_small(emb, Wt["temb_all.w"], temb_all, bias=Wt["temb_all.b"], act_in=1)
 
         # ---- geometry + concat buffers ------------------------------------------------------
-        res_hw = [(H >> i, W >> i) for i in range(L)]
+        # the stride-2 pad-1 Downsample2D conv gives ceil(s/2); the up path resizes back to each skip level's size
+        res_hw = [(H, W)]
+        for _ in range(L - 1):
+            res_hw.append(((res_hw[-1][0] + 1) // 2, (res_hw[-1][1] + 1) // 2))
 
         def rows_at(level):
             return B * res_hw[level][0] * res_hw[level][1]
@@ -670,9 +674,10 @@ class _Lowering:
             if i < L - 1:
                 nm = f"up_blocks.{i}.upsamplers.0.conv"
                 h_, w_ = res_hw[lvl]
+                ho, wo = res_hw[lvl - 1]
                 up = scratch("up", rows_at(lvl - 1), cout)
-                P.upsample2x(x, B, h_, w_, cout, up)
-                P.gemm(up, Wt[nm + ".w"], cout, B, 2 * h_, 2 * w_, cats[ci]["hidden"], taps=9, bias=Wt[nm + ".b"])
+                P.upsample2x(x, B, h_, w_, cout, up, ho, wo)
+                P.gemm(up, Wt[nm + ".w"], cout, B, ho, wo, cats[ci]["hidden"], taps=9, bias=Wt[nm + ".b"])
         # ---- out ----------------------------------------------------------------------------
         no = scratch("n1", rows_at(0), ch[0])
         P.groupnorm(x, B, H * W, ch[0], groups, Wt["conv_norm_out.g"], Wt["conv_norm_out.b"], 1e-5, 1, no, self.ws)

@@ -156,17 +156,20 @@ class _VAELowering:
         x2 = torch.empty(S, C0, **f16)
         resnet("mid_block.resnets.0", x, C0, C0, h, w, x2)
         # mid-block attention (single head, dim C0)
-        hn = sc("n1", S, C0)
+        # V^T and the scores take the keys as the GEMM's N, which must be a multiple of 8: hn and qk get S8 >= S rows,
+        # the extra ones zero (never written), so the extra V^T and score columns are exact zeros
+        S8 = -(-S // 8) * 8
+        hn = torch.zeros(S8, C0, **f16)
         P.groupnorm(x2, B, S, C0, groups, Wt["attn.norm.g"], Wt["attn.norm.b"], 1e-6, 0, hn, self.ws)
-        qk = torch.empty(S, 2 * C0, **f16)
+        qk = torch.zeros(S8, 2 * C0, **f16)
         P.gemm(hn, Wt["attn.qk.w"], 2 * C0, 1, 1, S, qk, bias=Wt["attn.qk.b"])
-        # P V contracts over the S keys, and the GEMM's K must be a multiple of 64: P and V^T get Sp >= S columns, the
-        # extra ones zero (never written), which adds exact zeros to every dot product
+        # P V contracts over the S keys, and the GEMM's K must be a multiple of 64: P and V^T get Sp >= S8 columns, the
+        # extra ones zero, which adds exact zeros to every dot product
         Sp = -(-S // 64) * 64
         vT = torch.zeros(C0, Sp, **f16)
-        P.gemm(Wt["attn.v.w"], hn, S, 1, 1, C0, vT[:, :S], static_w=False)               # V^T = Wv hn^T
+        P.gemm(Wt["attn.v.w"], hn, S8, 1, 1, C0, vT[:, :S8], static_w=False)             # V^T = Wv hn^T
         scores = torch.zeros(S, Sp, **f16)
-        P.gemm(qk[:, :C0], qk[:, C0:], S, 1, 1, S, scores[:, :S], static_w=False)        # (scaled q) k^T
+        P.gemm(qk[:, :C0], qk[:, C0:], S8, 1, 1, S, scores[:, :S8], static_w=False)      # (scaled q) k^T
         P.softmax_rows(scores[:, :S], scores[:, :S])
         att = sc("h1", S, C0)
         P.gemm(scores, vT, C0, 1, 1, S, att, static_w=False)                              # P V
@@ -198,5 +201,5 @@ class _VAELowering:
         else:
             P.conv_out(no, B, hh, ww, cin, Wt["conv_out.w"], Wt["conv_out.b"], 3, img)
         P.postprocess_u8(img, self.frame, vae.nonfinite)
-        self._keep = (scratch, z, qk, vT, scores, x2, x3, x4, img)
+        self._keep = (scratch, z, hn, qk, vT, scores, x2, x3, x4, img)
         P.finalize()

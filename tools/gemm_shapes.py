@@ -59,7 +59,9 @@ def unet_shapes(h=128, w=128):
         add("ff.out+res", hw, C, 4 * C, res=True, n=depth)
 
     ch, depth = (320, 640, 1280), (0, 2, 10)
-    hws = ((h, w), (h // 2, w // 2), (h // 4, w // 4))
+    hws = [(h, w)]
+    for _ in range(2):      # the stride-2 pad-1 downsample conv gives ceil(s/2)
+        hws.append(((hws[-1][0] + 1) // 2, (hws[-1][1] + 1) // 2))
     skips = [320]
     cin = 320
     for lvl in range(3):
