@@ -18,6 +18,14 @@
  *  - fp16 means IEEE binary16 (``__half``).  Activations are NHWC
  *    ([batch*height*width, channels] row-major); latents are NCHW like the
  *    reference's ``[1,4,h,w]`` tensors.
+ *  - bf16 means bfloat16 (``__nv_bfloat16``: fp32's 8-bit exponent, 8-bit
+ *    significand).  The VAE-decoder ops also exist in bf16 (LB_GEMM_BF16 and
+ *    the ``*_dt`` entry points with dtype LB_DTYPE_BF16): the stock SDXL VAE's
+ *    activations exceed fp16's range (the reference decodes it in fp32 when
+ *    its config sets force_upcast, diffusers_holder.py:128-139), bf16's range
+ *    is fp32's, and bf16 wgmma runs at the fp16 rate.  Every bf16 variant keeps
+ *    the fp16 variant's layouts, strides, alignment rules and fp32 arithmetic;
+ *    only the stored element type differs.
  */
 #ifndef LB200_H
 #define LB200_H
@@ -30,6 +38,9 @@ extern "C" {
 #endif
 
 #define LB_ABI_VERSION 2
+
+/* element type of the ops that exist in both 16-bit formats (lb_op.dtype, the ``*_dt`` entry points) */
+enum { LB_DTYPE_F16 = 0, LB_DTYPE_BF16 = 1 };
 
 typedef struct lb_ctx lb_ctx;
 
@@ -129,7 +140,7 @@ typedef struct lb_gemm_desc {
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
     int32_t mode;     /* low byte: 0 = linear epilogue, 1 = GEGLU; flags: LB_GEMM_STATIC_W, LB_GEMM_RELU,
-                         LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS */
+                         LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS, LB_GEMM_BF16, LB_GEMM_OUT_F16 */
     const void* ln_stats; int32_t ln_parts;      /* float2 [M][ln_parts] or NULL */
     const void* ln_csum; const void* ln_bias;    /* float [N] each */
     float ln_eps;
@@ -144,6 +155,13 @@ typedef struct lb_gemm_desc {
  * automatic choice; at most one of them */
 #define LB_GEMM_TILE_BOX 0x400
 #define LB_GEMM_TILE_RUNS 0x800
+/* mode flag: a0, a1, w, bias, bias2, res and out are bf16 instead of fp16 (fp32 accumulation as in fp16; the output
+ * is rounded to bf16).  Linear epilogue only: GEGLU, the LayerNorm fold and stats_out are rejected.  The VAE decoder of
+ * a checkpoint whose activations overflow fp16 runs on it. */
+#define LB_GEMM_BF16 0x1000
+/* mode flag, only with LB_GEMM_BF16: bf16 operands, fp16 output (the VAE attention scores, whose fp16 rounding is 8x
+ * finer than bf16's and whose magnitudes stay far inside fp16's range; lb_softmax_rows_dt reads them as fp16) */
+#define LB_GEMM_OUT_F16 0x2000
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
 /* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
  * that holds a row of the wgmma accumulator); < 0 on error */
@@ -180,6 +198,12 @@ size_t lb_groupnorm_workspace_bytes(lb_ctx* ctx, int B, int HW, int groups);
 int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
                  const void* gamma, const void* beta, float eps, int silu,
                  void* out, int64_t ldo, void* workspace, void* stream);
+/* lb_groupnorm with x, gamma, beta and out of element type ``dtype`` (LB_DTYPE_BF16: bf16, the same fp32 statistics
+ * and fixed-order reduction; the output is rounded to bf16 after the affine and again after SiLU).  lb_groupnorm is
+ * its LB_DTYPE_F16 call. */
+int lb_groupnorm_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
+                    const void* gamma, const void* beta, float eps, int silu,
+                    void* out, int64_t ldo, void* workspace, void* stream, int dtype);
 int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
                  const void* gamma, const void* beta, float eps, void* out, int64_t ldo, void* stream);
 
@@ -201,6 +225,10 @@ int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
  *   pixel (yo, xo) is input pixel (yo >> 1, xo >> 1), i.e. nearest 2x cropped to
  *   Ho x Wo.  lb_upsample2x is the Ho = 2H, Wo = 2W case.  C and both row strides
  *   multiples of 8.
+ * The ``*_dt`` variants take the element type as a trailing ``dtype``; the
+ *   plain entry points are their LB_DTYPE_F16 calls.  lb_conv_in_dt with
+ *   LB_DTYPE_BF16: x, w_packed, bias and out are bf16.  lb_upsample_nearest_dt
+ *   copies 16-byte channel vectors, so it is the same kernel for both types.
  */
 int lb_embed_inputs(lb_ctx* ctx, float t, const void* text_embeds, const void* time_ids, int B,
                     int dim_t, int pooled, int dim_a, void* temb_in, void* add_in, void* stream);
@@ -215,6 +243,10 @@ int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, i
                   void* stream);
 int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
                         int Ho, int Wo, void* stream);
+int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                  const void* bias, int Cout, void* out, int64_t ldo, void* stream, int dtype);
+int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                           int64_t ldo, int Ho, int Wo, void* stream, int dtype);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
 
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
@@ -226,6 +258,13 @@ int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, in
  *   (optional, device int) is incremented by the number of NaN/Inf pixels: the decoder runs in fp16 where the reference
  *   upcasts the stock SDXL VAE to fp32 because it "overflows in float16" (diffusers_holder.py:128-133); an overflow
  *   anywhere upstream reaches the image as Inf/NaN and is reported instead of silently producing a black frame.
+ * The ``*_dt`` variants take the element type as a trailing ``dtype`` (the plain entry points are their LB_DTYPE_F16
+ * calls).  With LB_DTYPE_BF16 (the bf16 decoder of a VAE that overflows fp16):
+ *   lb_latent_prep_dt: fp16 latents in, bf16 out;
+ *   lb_softmax_rows_dt: fp16 scores in (lb_gemm with LB_GEMM_BF16 | LB_GEMM_OUT_F16), bf16 probabilities out; in
+ *     place too (out == x, ldo == ld: every element is read before the same thread overwrites its 2 bytes);
+ *   lb_postprocess_u8_dt: bf16 image in; non-finite pixels are still counted;
+ *   lb_nhwc_to_nchw_dt: bf16 in and out.
  */
 int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
                    const void* bias_f32, void* out_nchw, void* stream);
@@ -233,11 +272,19 @@ int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int co
                     void* stream);
 int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
                       int* nonfinite_count_dev, void* stream);
+int lb_latent_prep_dt(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
+                      const void* bias_f32, void* out_nchw, void* stream, int dtype);
+int lb_softmax_rows_dt(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
+                       void* stream, int dtype);
+int lb_postprocess_u8_dt(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
+                         int* nonfinite_count_dev, void* stream, int dtype);
 /* lb_nhwc_to_nchw: the first C (<= 8) columns of NHWC rows [B*hw, ld] -> NCHW [B, C, hw].  The C0 -> 4 (UNet eps) and
  * C0 -> 3 (VAE RGB) output convolutions run as lb_gemm with an 8-row zero-padded weight matrix (N = 8); this puts the
  * result back into the reference's [B,C,H,W] tensor layout.  (lb_conv_out is the direct kernel for widths that are not
  * multiples of 64.) */
 int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream);
+int lb_nhwc_to_nchw_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream,
+                       int dtype);
 
 /* ---- LPIPS-AlexNet branch-placement metric (SURVEY section 8f next #2; blending_engine.py:744-758, lpips==0.1.4) ----
  * The five AlexNet convolutions run on lb_gemm (LB_GEMM_RELU) over patch matrices:
@@ -273,6 +320,9 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * lb_program_run replays it on ``stream`` (``t`` = the timestep fed to
  * LB_OP_EMBED_INPUTS).  Replaces the module walk of pipe.unet(...)
  * (diffusers_holder.py:336-344).
+ * lb_op.dtype: the element type (LB_DTYPE_*) of GROUPNORM, LATENT_PREP, CONV_IN, UPSAMPLE2X, NHWC_TO_NCHW,
+ * POSTPROCESS_U8 and SOFTMAX_ROWS (for SOFTMAX_ROWS the output's: see lb_softmax_rows_dt), i.e. which ``*_dt`` call
+ * the record makes.  It must be 0 for every other kind (a GEMM takes its types from its mode flags).
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
@@ -282,7 +332,7 @@ enum {
 };
 typedef struct lb_op {
     int32_t kind;
-    int32_t reserved;
+    int32_t dtype;      /* LB_DTYPE_F16 (0) or LB_DTYPE_BF16, see above */
     union {
         lb_gemm_desc gemm;
         lb_attn_desc attn;

@@ -90,13 +90,16 @@ class _OpUnion(ctypes.Union):
 
 class Op(ctypes.Structure):
     """lb_op of include/lb200.h."""
-    _fields_ = [("kind", c_int32), ("reserved", c_int32), ("u", _OpUnion)]
+    _fields_ = [("kind", c_int32), ("dtype", c_int32), ("u", _OpUnion)]
 
 
 GEMM_STATIC_W = 0x100     # lb_gemm_desc.mode flag (include/lb200.h: LB_GEMM_STATIC_W)
 GEMM_RELU = 0x200         # LB_GEMM_RELU
 GEMM_TILE_BOX = 0x400     # LB_GEMM_TILE_BOX: force the pixel-box M tiling
 GEMM_TILE_RUNS = 0x800    # LB_GEMM_TILE_RUNS: force the pixel-run M tiling
+GEMM_BF16 = 0x1000        # LB_GEMM_BF16: bf16 operands, bias, residual and output
+GEMM_OUT_F16 = 0x2000     # LB_GEMM_OUT_F16 (with GEMM_BF16): fp16 output
+DTYPE_F16, DTYPE_BF16 = 0, 1    # LB_DTYPE_F16 / LB_DTYPE_BF16: lb_op.dtype and the *_dt entry points
 (OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN, OP_CONV_OUT,
  OP_UPSAMPLE2X, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
  OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = range(1, 18)
@@ -130,6 +133,8 @@ SIGNATURES = {
     "lb_groupnorm_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int]),
     "lb_groupnorm": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
                              c_int, c_void_p, c_int64, c_void_p, c_void_p]),
+    "lb_groupnorm_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
+                                c_int, c_void_p, c_int64, c_void_p, c_void_p, c_int]),
     "lb_layernorm": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p,
                              c_int64, c_void_p]),
     "lb_embed_inputs": (c_int, [c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
@@ -138,16 +143,25 @@ SIGNATURES = {
                                 c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_void_p]),
     "lb_conv_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                            c_int64, c_void_p]),
+    "lb_conv_in_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                              c_int64, c_void_p, c_int]),
     "lb_conv_out": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                             c_void_p, c_void_p]),
     "lb_upsample2x": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
                                     c_int, c_void_p]),
+    "lb_upsample_nearest_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64,
+                                       c_int, c_int, c_void_p, c_int]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "lb_latent_prep": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "lb_softmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p]),
     "lb_postprocess_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     "lb_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_void_p, c_void_p]),
+    "lb_latent_prep_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_int]),
+    "lb_softmax_rows_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p, c_int]),
+    "lb_postprocess_u8_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int]),
+    "lb_nhwc_to_nchw_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_void_p, c_void_p, c_int]),
     "lb_lpips_im2col_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_float),
                                    ctypes.POINTER(c_float), c_void_p, c_int64, c_void_p]),
     "lb_im2col": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

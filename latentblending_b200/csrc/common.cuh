@@ -1,6 +1,7 @@
 // common.cuh -- shared host/device helpers for liblb200 (sm_90a only).
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -84,6 +85,28 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 #ifdef __CUDACC__
 // fp16 rounding of an fp32 value exactly as a torch fp16 op stores it
 __device__ __forceinline__ float lb_round_h(float x) { return __half2float(__float2half_rn(x)); }
+
+// The 16-bit storage types of the kernels that exist in fp16 and bf16 (LB_DTYPE_F16 / LB_DTYPE_BF16): the element
+// type T, its pair type, and fp32 <-> T conversions.  Both are 2 bytes, so vector widths and strides do not change.
+template <typename T> struct LbType;
+template <> struct LbType<__half> {
+    using T2 = __half2;
+    static __device__ __forceinline__ float to_f(__half v) { return __half2float(v); }
+    static __device__ __forceinline__ float2 to_f2(__half2 v) { return __half22float2(v); }
+    static __device__ __forceinline__ __half from_f(float v) { return __float2half_rn(v); }
+    static __device__ __forceinline__ __half2 from_f2(float a, float b) { return __floats2half2_rn(a, b); }
+    static __device__ __forceinline__ __half2 zero2() { return __float2half2_rn(0.f); }
+    static __device__ __forceinline__ float round(float v) { return lb_round_h(v); }
+};
+template <> struct LbType<__nv_bfloat16> {
+    using T2 = __nv_bfloat162;
+    static __device__ __forceinline__ float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
+    static __device__ __forceinline__ float2 to_f2(__nv_bfloat162 v) { return __bfloat1622float2(v); }
+    static __device__ __forceinline__ __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
+    static __device__ __forceinline__ __nv_bfloat162 from_f2(float a, float b) { return __floats2bfloat162_rn(a, b); }
+    static __device__ __forceinline__ __nv_bfloat162 zero2() { return __float2bfloat162_rn(0.f); }
+    static __device__ __forceinline__ float round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+};
 
 // 128-bit streaming load/store (read-once data: do not allocate in L1)
 __device__ __forceinline__ uint4 lb_ldg_stream(const void* p) {

@@ -35,9 +35,15 @@
 // Weight (B operand) tiles of the first pipeline stages are requested BEFORE
 // griddepcontrol.wait when the caller marks the weights static (LB_GEMM_STATIC_W):
 // their HBM latency hides behind the tail of the previous kernel.
+// Element type: fp16, or bf16 (LB_GEMM_BF16: the VAE decoder of a checkpoint whose activations overflow fp16) -- a
+// template parameter that changes only the TMA element type, the wgmma input type and the epilogue's loads / stores
+// (bf16 kernels: linear epilogue only; LB_GEMM_OUT_F16 stores fp16).  Both are 2 bytes, so boxes, swizzle, ring and
+// tilings are shared.
 // Bound: tensor pipe; algorithmic FLOPs = 2*M*N*K.
 #include "gemm_sm90.cuh"
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "sm90.cuh"
 
@@ -81,7 +87,9 @@ __device__ __forceinline__ float gelu_erf(float x) {
 }
 
 __device__ __forceinline__ float2 ld_f2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
-__device__ __forceinline__ __half2 ld_h2(const __half* p) { return __ldg(reinterpret_cast<const __half2*>(p)); }
+template <typename T> __device__ __forceinline__ typename LbType<T>::T2 ld_2(const T* p) {
+    return __ldg(reinterpret_cast<const typename LbType<T>::T2*>(p));
+}
 
 // (mu, rstd) of one row of the LayerNorm-folded A operand from the producer's per-row partial sums (fixed order).
 // The partials of a row are contiguous (<= 64 x float2): they are fetched as float4 pairs, eight loads in flight at
@@ -123,9 +131,14 @@ struct EpiRow {
 // 8j + 2*quad + e).  The global loads of a batch of column groups are all issued before any of its stores: the
 // residual may alias the output (in-place `hs += f(hs)`) and only this thread reads and writes these elements, so
 // the order is safe, and the loads overlap instead of costing one L2 round trip per 8-column group.
-template <int BN>
+// T: the element type of bias, bias2, res and out (bf16 kernels store fp16 instead when p.out_f16 is set); the
+// LayerNorm fold and stats_out exist in the fp16 kernels only.
+template <int BN, typename T>
 __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float (&acc)[BN / 2], const EpiRow (&r)[2],
                                                 int n_tile, int quad) {
+    using L = LbType<T>;
+    using T2 = typename L::T2;
+    constexpr bool kF16 = std::is_same<T, __half>::value;
     constexpr int G = BN / 8;                    // 8-column groups per row
     constexpr int CH = G > 10 ? G / 2 : G;       // groups per load batch (register budget)
     static_assert(G % CH == 0, "load batches must tile the row");
@@ -134,9 +147,9 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
     for (int i = 0; i < 2; ++i) {
         if (!r[i].ok) continue;
         float st_sum = 0.f, st_sq = 0.f;
-        const __half* res_row = p.res ? p.res + r[i].row * p.ldr : nullptr;
-        const __half* b2_row = p.bias2 ? p.bias2 + (long long)r[i].bidx * p.bias2_ld : nullptr;
-        __half* out_row = p.out + r[i].row * p.ldo;
+        const T* res_row = p.res ? reinterpret_cast<const T*>(p.res) + r[i].row * p.ldr : nullptr;
+        const T* b2_row = p.bias2 ? reinterpret_cast<const T*>(p.bias2) + (long long)r[i].bidx * p.bias2_ld : nullptr;
+        T* out_row = reinterpret_cast<T*>(p.out) + r[i].row * p.ldo;
 #pragma unroll
         for (int c0 = 0; c0 < G; c0 += CH) {
             float v[CH][2];
@@ -145,7 +158,7 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                 v[g][0] = acc[4 * (c0 + g) + 2 * i];
                 v[g][1] = acc[4 * (c0 + g) + 2 * i + 1];
             }
-            if (p.ln_stats) {
+            if (kF16 && p.ln_stats) {
                 constexpr int CL = CH > 8 ? CH / 2 : CH;     // fp32 vectors: half the batch
 #pragma unroll
                 for (int l0 = 0; l0 < CH; l0 += CL) {
@@ -163,30 +176,30 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                     }
                 }
             } else {
-                const __half2 z = __float2half2_rn(0.f);
-                __half2 hb[CH], hb2[CH], hr[CH];
+                const T2 z = L::zero2();
+                T2 hb[CH], hb2[CH], hr[CH];
 #pragma unroll
                 for (int g = 0; g < CH; ++g) {
                     const int n = n_base + 8 * (c0 + g);    // N is a multiple of 8 (checked on the host)
                     const bool in = n < p.N;
-                    hb[g] = (p.bias && in) ? ld_h2(p.bias + n) : z;
-                    hb2[g] = (b2_row && in) ? ld_h2(b2_row + n) : z;
-                    hr[g] = (res_row && in) ? *reinterpret_cast<const __half2*>(res_row + n) : z;
+                    hb[g] = (p.bias && in) ? ld_2(reinterpret_cast<const T*>(p.bias) + n) : z;
+                    hb2[g] = (b2_row && in) ? ld_2(b2_row + n) : z;
+                    hr[g] = (res_row && in) ? *reinterpret_cast<const T2*>(res_row + n) : z;
                 }
 #pragma unroll
                 for (int g = 0; g < CH; ++g) {
                     if (p.bias) {
-                        const float2 t = __half22float2(hb[g]);
+                        const float2 t = L::to_f2(hb[g]);
                         v[g][0] += t.x;
                         v[g][1] += t.y;
                     }
                     if (b2_row) {
-                        const float2 t = __half22float2(hb2[g]);
+                        const float2 t = L::to_f2(hb2[g]);
                         v[g][0] += t.x;
                         v[g][1] += t.y;
                     }
                     if (res_row) {
-                        const float2 t = __half22float2(hr[g]);
+                        const float2 t = L::to_f2(hr[g]);
                         v[g][0] += t.x;
                         v[g][1] += t.y;
                     }
@@ -201,17 +214,23 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                         v0 = fmaxf(v0, 0.f);
                         v1 = fmaxf(v1, 0.f);
                     }
-                    const __half2 o = __floats2half2_rn(v0, v1);
-                    *reinterpret_cast<__half2*>(out_row + n) = o;
-                    if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
-                        const float2 f = __half22float2(o);
-                        st_sum += f.x + f.y;
-                        st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
+                    if constexpr (kF16) {
+                        const __half2 o = __floats2half2_rn(v0, v1);
+                        *reinterpret_cast<__half2*>(out_row + n) = o;
+                        if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
+                            const float2 f = __half22float2(o);
+                            st_sum += f.x + f.y;
+                            st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
+                        }
+                    } else if (p.out_f16) {      // the same 2-byte element address, fp16 value
+                        *reinterpret_cast<__half2*>(out_row + n) = __floats2half2_rn(v0, v1);
+                    } else {
+                        *reinterpret_cast<T2*>(out_row + n) = L::from_f2(v0, v1);
                     }
                 }
             }
         }
-        if (p.stats_out)
+        if (kF16 && p.stats_out)
             p.stats_out[r[i].row * (kEpiParts * p.tiles_n) + kEpiParts * n_tile + quad] = make_float2(st_sum, st_sq);
     }
 }
@@ -255,8 +274,8 @@ __device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float 
         } else {
 #pragma unroll
             for (int j = 0; j < G; ++j) {
-                bv[j] = p.bias ? __half22float2(ld_h2(p.bias + a_base + 8 * j)) : make_float2(0.f, 0.f);
-                bg[j] = p.bias ? __half22float2(ld_h2(p.bias + a_base + HN + 8 * j)) : make_float2(0.f, 0.f);
+                bv[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + 8 * j)) : make_float2(0.f, 0.f);
+                bg[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + HN + 8 * j)) : make_float2(0.f, 0.f);
             }
 #pragma unroll
             for (int j = 0; j < G; ++j) {
@@ -270,10 +289,12 @@ __device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float 
     }
 }
 
-// kRuns: pixel-run M tiles (p.runs = 1); a separate instantiation, so the pixel-box kernels stay as they were
-template <int BN, bool kRuns>
+// kRuns: pixel-run M tiles (p.runs = 1); a separate instantiation, so the pixel-box kernels stay as they were.
+// T: operand / epilogue element type, __half or __nv_bfloat16 (LB_GEMM_BF16; linear epilogue only).
+template <int BN, bool kRuns, typename T>
 __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
     using C = Cfg<BN>;
+    constexpr bool kF16 = std::is_same<T, __half>::value;
     constexpr int nst = C::stages;
     constexpr bool kCoop = C::coop;
     pdl_launch_dependents();       // the next kernel may start its launch + prologue while this one runs
@@ -424,7 +445,7 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
             for (int i = 0; i < 2; ++i) {
                 ln_mu[hh][i] = 0.f;
                 ln_rstd[hh][i] = 1.f;
-                if (p.ln_stats) {
+                if (kF16 && p.ln_stats) {
                     row_of(hh, i);
                     ln_row_stats(p, er[hh][i].row, er[hh][i].ok, ln_mu[hh][i], ln_rstd[hh][i]);
                 }
@@ -461,7 +482,7 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
                 const uint64_t bdesc = make_smem_desc_sw128(b_addr + k * 32, 16, 1024);
 #pragma unroll
                 for (int hh = 0; hh < kHalves; ++hh)
-                    WgmmaSS<BN>::template mma<0>(acc[hh],
+                    WgmmaSS<BN>::template mma<0, !kF16>(acc[hh],
                                                  make_smem_desc_sw128(a_addr + half_of(hh) * (64 * 128) + k * 32, 16,
                                                                       1024),
                                                  bdesc, (kb | k) != 0);
@@ -501,8 +522,8 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
         for (int hh = 0; hh < kHalves; ++hh) {
             if constexpr (kRuns) rows_of_half(hh);
-            if (p.mode == 0) epilogue_linear<BN>(p, acc[hh], er[hh], n_tile, quad);
-            else if constexpr (BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
+            if (p.mode == 0) epilogue_linear<BN, T>(p, acc[hh], er[hh], n_tile, quad);
+            else if constexpr (kF16 && BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
         }
     }
 }
@@ -525,9 +546,14 @@ int get_encode(lb_ctx* ctx, EncodeTiledFn* fn) {
     return 0;
 }
 
+// TMA element type of the fp16 / bf16 kernels (both 2 bytes: boxes, strides and the swizzle are the same)
+CUtensorMapDataType tma_dtype(bool bf16) {
+    return bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+
 // 4-D NHWC activation map: dims (C, W, H, B), box (64, tw, th, tb), 128B swizzle, zero OOB fill.
 int encode_act_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int C, int W, int H, int B, int tw,
-                   int th, int tb) {
+                   int th, int tb, bool bf16) {
     EncodeTiledFn enc;
     if (int e = get_encode(ctx, &enc)) return e;
     LB_REQUIRE(lb_aligned16(base), "activation base must be 16-byte aligned");
@@ -536,7 +562,7 @@ int encode_act_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, in
     cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)ld * 2 * W, (cuuint64_t)ld * 2 * W * H};
     cuuint32_t box[4] = {(cuuint32_t)kBK, (cuuint32_t)tw, (cuuint32_t)th, (cuuint32_t)tb};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+    CUresult r = enc(m, tma_dtype(bf16), 4, const_cast<void*>(base), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(activation C=%d W=%d H=%d B=%d ld=%lld box=%d,%d,%d) failed: %d",
@@ -566,7 +592,8 @@ int get_encode_im2col(lb_ctx* ctx, EncodeIm2colFn* fn) {
 // per image, so a run of 128 consecutive box positions is 128 consecutive output pixels.  The position of output pixel
 // (x, y) is (x - 1, y - 1); with im2col offset (dx + 1, dy + 1) it reads input pixel (x + dx, y + dy), the 3x3 tap
 // (dy, dx) at padding 1 (a 1x1 segment uses offset (1, 1)).
-int encode_act_map_runs(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int C, int W, int H, int B) {
+int encode_act_map_runs(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int C, int W, int H, int B,
+                        bool bf16) {
     EncodeIm2colFn enc;
     if (int e = get_encode_im2col(ctx, &enc)) return e;
     LB_REQUIRE(lb_aligned16(base), "activation base must be 16-byte aligned");
@@ -575,7 +602,7 @@ int encode_act_map_runs(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t l
     cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)ld * 2 * W, (cuuint64_t)ld * 2 * W * H};
     const int lower[2] = {-1, -1}, upper[2] = {-1, -1};     // (W, H)
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, lower, upper,
+    CUresult r = enc(m, tma_dtype(bf16), 4, const_cast<void*>(base), dims, strides, lower, upper,
                      (cuuint32_t)kBK, (cuuint32_t)kBM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col(activation C=%d W=%d H=%d B=%d ld=%lld) failed: %d", C, W, H,
@@ -583,7 +610,7 @@ int encode_act_map_runs(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t l
     return 0;
 }
 
-int encode_weight_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int64_t K, int N, int bn) {
+int encode_weight_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld, int64_t K, int N, int bn, bool bf16) {
     EncodeTiledFn enc;
     if (int e = get_encode(ctx, &enc)) return e;
     LB_REQUIRE(lb_aligned16(base), "weight base must be 16-byte aligned");
@@ -592,7 +619,7 @@ int encode_weight_map(lb_ctx* ctx, CUtensorMap* m, const void* base, int64_t ld,
     cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
     cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)bn};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+    CUresult r = enc(m, tma_dtype(bf16), 2, const_cast<void*>(base), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     LB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(weight K=%lld N=%d bn=%d) failed: %d", (long long)K, N, bn,
@@ -619,20 +646,24 @@ const char* box_tiling(const GemmDesc& d, int* tw, int* th, int* tb) {
     return nullptr;
 }
 
-template <int BN, bool kRuns> int launch_tiled(const GemmPlan& plan, cudaStream_t st) {
+template <int BN, bool kRuns, typename T> int launch_tiled(const GemmPlan& plan, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, kRuns>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, kRuns, T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            Cfg<BN>::smem_bytes));
         attr_set = true;
     }
-    LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN, kRuns>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
+    LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN, kRuns, T>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
                                 (size_t)Cfg<BN>::smem_bytes, st, plan.p));
     return 0;
 }
 
+template <int BN, typename T> int launch_bn_t(const GemmPlan& plan, cudaStream_t st) {
+    return plan.p.runs ? launch_tiled<BN, true, T>(plan, st) : launch_tiled<BN, false, T>(plan, st);
+}
+
 template <int BN> int launch_bn(const GemmPlan& plan, cudaStream_t st) {
-    return plan.p.runs ? launch_tiled<BN, true>(plan, st) : launch_tiled<BN, false>(plan, st);
+    return plan.bf16 ? launch_bn_t<BN, __nv_bfloat16>(plan, st) : launch_bn_t<BN, __half>(plan, st);
 }
 
 }  // namespace
@@ -651,8 +682,17 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     LB_REQUIRE(!d.bias2 || (lb_aligned16(d.bias2) && d.bias2_ld % 8 == 0), "gemm: bias2 alignment");
     GemmParams& p = plan->p;
     memset(&p, 0, sizeof(p));
-    LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS)) == 0,
+    LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 |
+                           LB_GEMM_OUT_F16)) == 0,
                "gemm: unknown mode flags 0x%x", d.mode);
+    const bool bf16 = (d.mode & LB_GEMM_BF16) != 0;
+    LB_REQUIRE(bf16 || !(d.mode & LB_GEMM_OUT_F16), "gemm: LB_GEMM_OUT_F16 needs LB_GEMM_BF16");
+    if (bf16) {
+        LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_BF16 supports the linear epilogue only (no GEGLU)");
+        LB_REQUIRE(!d.ln_stats, "gemm: LB_GEMM_BF16 does not support the LayerNorm fold");
+        LB_REQUIRE(!d.stats_out, "gemm: LB_GEMM_BF16 does not support stats_out");
+    }
+    plan->bf16 = bf16;
     const int force = d.mode & (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS);
     LB_REQUIRE(force != (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS), "gemm: LB_GEMM_TILE_BOX and LB_GEMM_TILE_RUNS exclude "
                "each other");
@@ -728,8 +768,8 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     p.total_kb = total;
     const int64_t Ktot = (int64_t)total * kBK;
     const auto encode_a = [&](CUtensorMap* m, const void* base, int64_t ld, int c) {
-        return runs ? encode_act_map_runs(ctx, m, base, ld, c, d.W, d.H, d.B)
-                    : encode_act_map(ctx, m, base, ld, c, d.W, d.H, d.B, tw, th, tb);
+        return runs ? encode_act_map_runs(ctx, m, base, ld, c, d.W, d.H, d.B, bf16)
+                    : encode_act_map(ctx, m, base, ld, c, d.W, d.H, d.B, tw, th, tb, bf16);
     };
     if (int e = encode_a(&p.tmA[0], d.a0, d.a0_ld, d.a0_c)) return e;
     if (d.a1) {
@@ -737,9 +777,10 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     } else {
         p.tmA[1] = p.tmA[0];
     }
-    if (int e = encode_weight_map(ctx, &p.tmB, d.w, d.w_ld, Ktot, d.N, bn)) return e;
+    if (int e = encode_weight_map(ctx, &p.tmB, d.w, d.w_ld, Ktot, d.N, bn, bf16)) return e;
     p.out = static_cast<__half*>(d.out);
     p.ldo = d.out_ld;
+    p.out_f16 = (d.mode & LB_GEMM_OUT_F16) ? 1 : 0;
     p.bias = static_cast<const __half*>(d.bias);
     p.bias2 = static_cast<const __half*>(d.bias2);
     p.bias2_ld = d.bias2_ld;

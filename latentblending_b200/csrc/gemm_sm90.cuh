@@ -15,7 +15,7 @@ struct GemmDesc {
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
     int32_t mode;   // low byte: 0 linear epilogue, 1 GEGLU (N accumulators -> N/2 outputs); | LB_GEMM_STATIC_W | LB_GEMM_RELU
-                    // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS
+                    // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 | LB_GEMM_OUT_F16
     // LayerNorm folded into this GEMM (see include/lb200.h)
     const void* ln_stats; int32_t ln_parts;
     const void* ln_csum; const void* ln_bias; float ln_eps;
@@ -36,6 +36,7 @@ struct alignas(64) GemmParams {
     int N;
     int mode;
     int static_w;  // weights may be fetched before griddepcontrol.wait (LB_GEMM_STATIC_W)
+    // fp16, or bf16 in the bf16 instantiations (LB_GEMM_BF16), which reinterpret these pointers
     __half* out; long long ldo;
     const __half* bias;
     const __half* bias2; long long bias2_ld;
@@ -51,11 +52,13 @@ struct alignas(64) GemmParams {
     // (it may span image rows and images; M = B*H*W < 2^31), loaded by TMA im2col runs
     int runs;
     int M, HW;
+    int out_f16;   // bf16 instantiations: the output is stored as fp16 (LB_GEMM_OUT_F16)
 };
 
 struct GemmPlan {
     GemmParams p;
-    int bn;        // N tile: 64 / 128 / 160
+    int bn;        // N tile: 64 / 128 / 160 / 256
+    bool bf16;     // operands, bias, residual (and, unless p.out_f16, the output) are bf16
     int grid;
 };
 

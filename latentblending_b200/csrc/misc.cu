@@ -109,13 +109,16 @@ linear_small_kernel(const __half* __restrict__ x, long long ldx, int M, int K, c
 }
 
 // ---- conv_in: NCHW [B,Cin<=8,H,W] -> NHWC [B*H*W, Cout], 3x3 pad 1 -------------------------------
-// weights packed [ky][kx][cin][Cout] fp16 so a lane reads 8 consecutive output channels.
+// weights packed [ky][kx][cin][Cout] fp16 (bf16 in the bf16 variant) so a lane reads 8 consecutive output channels.
+template <typename T>
 __global__ void __launch_bounds__(kThreads)
-conv_in_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const __half* __restrict__ wp,
-               const __half* __restrict__ bias, int Cout, __half* __restrict__ out, long long ldo) {
+conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* __restrict__ wp,
+               const T* __restrict__ bias, int Cout, T* __restrict__ out, long long ldo) {
+    using L = LbType<T>;
     pdl_launch_dependents();
     pdl_wait();
-    extern __shared__ __half s_w[];   // [9*Cin][Cout]
+    extern __shared__ __half s_w_raw[];
+    T* s_w = reinterpret_cast<T*>(s_w_raw);   // [9*Cin][Cout] (T is 2 bytes, like __half)
     const int wn = 9 * Cin * Cout;
     for (int i = threadIdx.x; i < wn; i += kThreads) s_w[i] = wp[i];
     __syncthreads();
@@ -129,10 +132,10 @@ conv_in_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const
             float acc[8];
             {
                 const uint4 bv = *reinterpret_cast<const uint4*>(bias + g * 8);
-                const __half2* bh = reinterpret_cast<const __half2*>(&bv);
+                const auto* bh = reinterpret_cast<const typename L::T2*>(&bv);
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const float2 f = __half22float2(bh[j]);
+                    const float2 f = L::to_f2(bh[j]);
                     acc[2 * j] = f.x;
                     acc[2 * j + 1] = f.y;
                 }
@@ -144,12 +147,12 @@ conv_in_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const
                     const int xx = xw + kx - 1;
                     if (xx < 0 || xx >= W) continue;
                     for (int c = 0; c < Cin; ++c) {
-                        const float xv = __half2float(x[(((long long)b * Cin + c) * H + yy) * W + xx]);
+                        const float xv = L::to_f(x[(((long long)b * Cin + c) * H + yy) * W + xx]);
                         const uint4 wv = *reinterpret_cast<const uint4*>(s_w + ((ky * 3 + kx) * Cin + c) * Cout + g * 8);
-                        const __half2* wh = reinterpret_cast<const __half2*>(&wv);
+                        const auto* wh = reinterpret_cast<const typename L::T2*>(&wv);
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {
-                            const float2 f = __half22float2(wh[j]);
+                            const float2 f = L::to_f2(wh[j]);
                             acc[2 * j] = fmaf(xv, f.x, acc[2 * j]);
                             acc[2 * j + 1] = fmaf(xv, f.y, acc[2 * j + 1]);
                         }
@@ -157,9 +160,9 @@ conv_in_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const
                 }
             }
             uint4 o;
-            __half2* oh = reinterpret_cast<__half2*>(&o);
+            auto* oh = reinterpret_cast<typename L::T2*>(&o);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(acc[2 * j], acc[2 * j + 1]);
+            for (int j = 0; j < 4; ++j) oh[j] = L::from_f2(acc[2 * j], acc[2 * j + 1]);
             *reinterpret_cast<uint4*>(out + pix * ldo + g * 8) = o;
         }
     }
@@ -315,7 +318,8 @@ extern "C" int lb_linear_small(lb_ctx* ctx, const void* x, int64_t ldx, int M, i
     return 0;
 }
 
-extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+template <typename T>
+static int conv_in_launch(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
                           const void* bias, int Cout, void* out, int64_t ldo, void* stream) {
     LB_REQUIRE(ctx && x_nchw && w_packed && bias && out, "lb_conv_in: null argument");
     LB_REQUIRE(Cin >= 1 && Cin <= 8 && Cout % 8 == 0 && ldo % 8 == 0, "lb_conv_in: Cin<=8, Cout%%8==0 required");
@@ -323,17 +327,29 @@ extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H
     LB_REQUIRE(smem <= 96 * 1024, "lb_conv_in: weights do not fit shared memory");
     static bool attr = false;
     if (!attr) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_in_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         attr = true;
     }
     const long long npix = (long long)B * H * W;
     unsigned grid = (unsigned)lb_ceil_div(npix, kThreads / 32);
     if (grid > (unsigned)ctx->sm_count * 4) grid = ctx->sm_count * 4;
-    lb_launch_pdl(conv_in_kernel, grid, kThreads, smem, lb_stream(stream), (const __half*)x_nchw, B, Cin, H, W,
-                                                               (const __half*)w_packed, (const __half*)bias, Cout,
-                                                               (__half*)out, ldo);
+    lb_launch_pdl(conv_in_kernel<T>, grid, kThreads, smem, lb_stream(stream), (const T*)x_nchw, B, Cin, H, W,
+                  (const T*)w_packed, (const T*)bias, Cout, (T*)out, ldo);
     LB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                             const void* bias, int Cout, void* out, int64_t ldo, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_conv_in: unknown dtype %d", dtype);
+    return dtype == LB_DTYPE_BF16
+               ? conv_in_launch<__nv_bfloat16>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream)
+               : conv_in_launch<__half>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream);
+}
+
+extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                          const void* bias, int Cout, void* out, int64_t ldo, void* stream) {
+    return lb_conv_in_dt(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream, LB_DTYPE_F16);
 }
 
 extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,
@@ -357,8 +373,10 @@ extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Ci
     return 0;
 }
 
-extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
-                                   int64_t ldo, int Ho, int Wo, void* stream) {
+// the kernel moves 16-byte channel vectors, so fp16 and bf16 maps share it
+extern "C" int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                                      int64_t ldo, int Ho, int Wo, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_upsample_nearest: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x && out, "lb_upsample_nearest: null argument");
     LB_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0, "lb_upsample_nearest: C and strides must be multiples of 8");
     LB_REQUIRE((Ho == 2 * H || Ho == 2 * H - 1) && (Wo == 2 * W || Wo == 2 * W - 1) && Ho >= 1 && Wo >= 1,
@@ -369,6 +387,11 @@ extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B
                   (const __half*)x, ld, B, H, W, C, (__half*)out, ldo, Ho, Wo);
     LB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                                   int64_t ldo, int Ho, int Wo, void* stream) {
+    return lb_upsample_nearest_dt(ctx, x, ld, B, H, W, C, out, ldo, Ho, Wo, stream, LB_DTYPE_F16);
 }
 
 extern "C" int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
@@ -388,11 +411,12 @@ extern "C" int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H
 
 // ======================= VAE-decoder helpers (SURVEY section 8f "next #1") ==========================================
 // latent_prep: z = post_quant_conv(latents / scaling_factor), a per-pixel CxC matrix (diffusers_holder.py:135,
-// AutoencoderKL.decode); NCHW fp16 in/out, the 1/scaling_factor is folded into w on the host.
+// AutoencoderKL.decode); NCHW fp16 in, fp16 or bf16 (TO) out, the 1/scaling_factor is folded into w on the host.
 namespace {
+template <typename TO>
 __global__ void __launch_bounds__(kThreads)
 latent_prep_kernel(const __half* __restrict__ x, int B, int C, long long hw, const float* __restrict__ w /*[C][C]*/,
-                   const float* __restrict__ bias, __half* __restrict__ out) {
+                   const float* __restrict__ bias, TO* __restrict__ out) {
     pdl_launch_dependents();
     pdl_wait();
     const long long total = (long long)B * hw;
@@ -403,20 +427,23 @@ latent_prep_kernel(const __half* __restrict__ x, int B, int C, long long hw, con
         for (int o = 0; o < C; ++o) {
             float acc = bias[o];
             for (int c = 0; c < C; ++c) acc = fmaf(w[o * C + c], in[c], acc);
-            out[(b * C + o) * hw + p] = __float2half_rn(acc);
+            out[(b * C + o) * hw + p] = LbType<TO>::from_f(acc);
         }
     }
 }
 
 // row softmax (in place capable): out[r,:] = softmax(x[r,:]) over `cols` fp16 values, one CTA per row.  Columns past
 // the last multiple of 8 (h*w keys of a VAE latent with an odd side) take a scalar tail after the 128-bit loop.
+// TO: the output type (fp16, or bf16 for the bf16 decoder's P); both are 2 bytes, so in place stays in place.
+template <typename TO>
 __global__ void __launch_bounds__(kThreads)
-softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half* __restrict__ out, long long ldo) {
+softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, TO* __restrict__ out, long long ldo) {
+    using L = LbType<TO>;
     pdl_launch_dependents();
     pdl_wait();
     const long long r = blockIdx.x;
     const __half* xr = x + r * ld;
-    __half* orow = out + r * ldo;
+    TO* orow = out + r * ldo;
     __shared__ float red[kThreads / 32];
     __shared__ float bc;
     const int vecs = cols >> 3;
@@ -468,16 +495,16 @@ softmax_rows_kernel(const __half* __restrict__ x, long long ld, int cols, __half
         const uint4 q = *reinterpret_cast<const uint4*>(xr + v * 8);
         const __half2* h = reinterpret_cast<const __half2*>(&q);
         uint4 o;
-        __half2* oh = reinterpret_cast<__half2*>(&o);
+        auto* oh = reinterpret_cast<typename L::T2*>(&o);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const float2 f = __half22float2(h[j]);
-            oh[j] = __floats2half2_rn(__expf(f.x - mx) * inv, __expf(f.y - mx) * inv);
+            oh[j] = L::from_f2(__expf(f.x - mx) * inv, __expf(f.y - mx) * inv);
         }
         *reinterpret_cast<uint4*>(orow + v * 8) = o;
     }
     for (int c = (vecs << 3) + threadIdx.x; c < cols; c += kThreads)
-        orow[c] = __float2half_rn(__expf(__half2float(xr[c]) - mx) * inv);
+        orow[c] = L::from_f(__expf(__half2float(xr[c]) - mx) * inv);
 }
 
 // NHWC rows [B*hw, ld] (first C columns) -> NCHW [B, C, hw]: the boundary of the conv_out GEMM (C = 4 eps / 3 RGB
@@ -498,8 +525,9 @@ nhwc_to_nchw_kernel(const __half* __restrict__ x, long long ld, int B, int C, lo
 // VaeImageProcessor.postprocess: NCHW fp16 image -> uint8 NHWC, (x/2+0.5).clamp(0,1)*255 rounded half-to-even.
 // `nonfinite` (optional) counts NaN/Inf pixels: the decoder runs in fp16 where the reference upcasts the stock SDXL VAE
 // to fp32 ("overflows in float16", diffusers_holder.py:128); an overflow anywhere upstream reaches the image as Inf/NaN.
+template <typename T>
 __global__ void __launch_bounds__(kThreads)
-postprocess_u8_kernel(const __half* __restrict__ img, int B, int C, long long hw, uint8_t* __restrict__ out,
+postprocess_u8_kernel(const T* __restrict__ img, int B, int C, long long hw, uint8_t* __restrict__ out,
                       int* __restrict__ nonfinite) {
     pdl_launch_dependents();
     pdl_wait();
@@ -508,7 +536,7 @@ postprocess_u8_kernel(const __half* __restrict__ img, int B, int C, long long hw
     for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
         const int c = (int)(i % C);
         const long long p = (i / C) % hw, b = i / (C * hw);
-        const float raw = __half2float(img[(b * C + c) * hw + p]);
+        const float raw = LbType<T>::to_f(img[(b * C + c) * hw + p]);
         bad += !isfinite(raw);
         float v = raw / 2.0f + 0.5f;
         v = fminf(fmaxf(v, 0.f), 1.f);
@@ -521,30 +549,54 @@ postprocess_u8_kernel(const __half* __restrict__ img, int B, int C, long long hw
 }
 }  // namespace
 
-extern "C" int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
-                              const void* bias_f32, void* out_nchw, void* stream) {
+extern "C" int lb_latent_prep_dt(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
+                                 const void* bias_f32, void* out_nchw, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_latent_prep: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x_nchw && w_f32 && bias_f32 && out_nchw, "lb_latent_prep: null argument");
     LB_REQUIRE(C >= 1 && C <= 8, "lb_latent_prep: C must be <= 8");
-    lb_launch_pdl(latent_prep_kernel, grid_for((long long)B * hw, ctx->sm_count), kThreads, 0, lb_stream(stream), 
-        (const __half*)x_nchw, B, C, hw, (const float*)w_f32, (const float*)bias_f32, (__half*)out_nchw);
+    const unsigned grid = grid_for((long long)B * hw, ctx->sm_count);
+    if (dtype == LB_DTYPE_BF16)
+        lb_launch_pdl(latent_prep_kernel<__nv_bfloat16>, grid, kThreads, 0, lb_stream(stream), (const __half*)x_nchw, B,
+                      C, hw, (const float*)w_f32, (const float*)bias_f32, (__nv_bfloat16*)out_nchw);
+    else
+        lb_launch_pdl(latent_prep_kernel<__half>, grid, kThreads, 0, lb_stream(stream), (const __half*)x_nchw, B, C, hw,
+                      (const float*)w_f32, (const float*)bias_f32, (__half*)out_nchw);
+    LB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
+                              const void* bias_f32, void* out_nchw, void* stream) {
+    return lb_latent_prep_dt(ctx, x_nchw, B, C, hw, w_f32, bias_f32, out_nchw, stream, LB_DTYPE_F16);
+}
+
+extern "C" int lb_softmax_rows_dt(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out,
+                                  int64_t ldo, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_softmax_rows: unknown dtype %d", dtype);
+    LB_REQUIRE(ctx && x && out, "lb_softmax_rows: null argument");
+    LB_REQUIRE(cols >= 0 && ld % 8 == 0 && ldo % 8 == 0 && lb_aligned16(x) && lb_aligned16(out),
+               "lb_softmax_rows: strides must be multiples of 8, bases 16B aligned");
+    LB_REQUIRE(rows <= 2147483647LL, "lb_softmax_rows: too many rows");
+    if (rows == 0) return 0;
+    if (dtype == LB_DTYPE_BF16)
+        lb_launch_pdl(softmax_rows_kernel<__nv_bfloat16>, (unsigned)rows, kThreads, 0, lb_stream(stream),
+                      (const __half*)x, ld, cols, (__nv_bfloat16*)out, ldo);
+    else
+        lb_launch_pdl(softmax_rows_kernel<__half>, (unsigned)rows, kThreads, 0, lb_stream(stream), (const __half*)x, ld,
+                      cols, (__half*)out, ldo);
     LB_LAUNCH_CHECK();
     return 0;
 }
 
 extern "C" int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
                                void* stream) {
-    LB_REQUIRE(ctx && x && out, "lb_softmax_rows: null argument");
-    LB_REQUIRE(cols >= 0 && ld % 8 == 0 && ldo % 8 == 0 && lb_aligned16(x) && lb_aligned16(out),
-               "lb_softmax_rows: strides must be multiples of 8, bases 16B aligned");
-    LB_REQUIRE(rows <= 2147483647LL, "lb_softmax_rows: too many rows");
-    if (rows == 0) return 0;
-    lb_launch_pdl(softmax_rows_kernel, (unsigned)rows, kThreads, 0, lb_stream(stream), (const __half*)x, ld, cols, (__half*)out, ldo);
-    LB_LAUNCH_CHECK();
-    return 0;
+    return lb_softmax_rows_dt(ctx, x, ld, rows, cols, out, ldo, stream, LB_DTYPE_F16);
 }
 
-extern "C" int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
-                               void* stream) {
+// copies 2-byte elements: the same kernel for fp16 and bf16
+extern "C" int lb_nhwc_to_nchw_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
+                                  void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_nhwc_to_nchw: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x && out_nchw, "lb_nhwc_to_nchw: null argument");
     LB_REQUIRE(C >= 1 && C <= 8 && ld % 8 == 0 && ld >= 8 && lb_aligned16(x), "lb_nhwc_to_nchw: C <= 8, row stride a "
                "multiple of 8 elements, 16B aligned base");
@@ -554,11 +606,27 @@ extern "C" int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, in
     return 0;
 }
 
-extern "C" int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
-                                 int* nonfinite_count_dev, void* stream) {
+extern "C" int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
+                               void* stream) {
+    return lb_nhwc_to_nchw_dt(ctx, x, ld, B, C, hw, out_nchw, stream, LB_DTYPE_F16);
+}
+
+extern "C" int lb_postprocess_u8_dt(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
+                                    int* nonfinite_count_dev, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_postprocess_u8: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && img_nchw && out_u8_nhwc, "lb_postprocess_u8: null argument");
-    lb_launch_pdl(postprocess_u8_kernel, grid_for((long long)B * hw * C, ctx->sm_count), kThreads, 0, lb_stream(stream), 
-        (const __half*)img_nchw, B, C, hw, (uint8_t*)out_u8_nhwc, nonfinite_count_dev);
+    const unsigned grid = grid_for((long long)B * hw * C, ctx->sm_count);
+    if (dtype == LB_DTYPE_BF16)
+        lb_launch_pdl(postprocess_u8_kernel<__nv_bfloat16>, grid, kThreads, 0, lb_stream(stream),
+                      (const __nv_bfloat16*)img_nchw, B, C, hw, (uint8_t*)out_u8_nhwc, nonfinite_count_dev);
+    else
+        lb_launch_pdl(postprocess_u8_kernel<__half>, grid, kThreads, 0, lb_stream(stream), (const __half*)img_nchw, B, C,
+                      hw, (uint8_t*)out_u8_nhwc, nonfinite_count_dev);
     LB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
+                                 int* nonfinite_count_dev, void* stream) {
+    return lb_postprocess_u8_dt(ctx, img_nchw, B, C, hw, out_u8_nhwc, nonfinite_count_dev, stream, LB_DTYPE_F16);
 }

@@ -8,7 +8,8 @@
 // Deterministic and batch-invariant: fixed-order reductions, no floating-point atomics (one integer
 // "last block" counter per batch element finalises the statistics).  fp32 statistics, fp64 final
 // combine; output rounded to fp16 after the affine and again after SiLU, like the
-// reference's two separate torch ops.
+// reference's two separate torch ops.  GroupNorm also exists in bf16 (the bf16 VAE decoder): same statistics and
+// summation order, bf16 loads and roundings.
 #include "common.cuh"
 
 namespace {
@@ -26,8 +27,9 @@ __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)
 
 // pass 1: per (batch, row-chunk) partial sums per group; the last chunk of a batch element to finish turns the
 // partials into (mean, rstd) per group -- fixed summation order, fp64 combine, no floating-point atomics.
+template <typename T>
 __global__ void __launch_bounds__(kThreads)
-gn_partial_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int groups, int rows_per_chunk,
+gn_partial_kernel(const T* __restrict__ x, long long ld, int C, int HW, int groups, int rows_per_chunk,
                   float eps, float2* __restrict__ partial /*[B][chunks][groups]*/,
                   float2* __restrict__ stats /*[B][groups] (mean, rstd)*/, int* __restrict__ counter /*[B]*/) {
     pdl_launch_dependents();
@@ -41,7 +43,7 @@ gn_partial_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int
     __shared__ int s_last;
     for (int c = threadIdx.x; c < C; c += kThreads) s_sum[c] = s_sq[c] = 0.f;
     __syncthreads();
-    const __half* base = x + ((long long)b * HW) * ld;
+    const T* base = x + ((long long)b * HW) * ld;
     const int RL = VP <= kThreads ? kThreads / VP : 1;
     for (int cv0 = 0; cv0 < VP; cv0 += kThreads) {          // one trip unless C > 2048
         const int cv = cv0 + (VP <= kThreads ? (int)threadIdx.x % VP : (int)threadIdx.x);
@@ -51,14 +53,14 @@ gn_partial_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int
 #pragma unroll
         for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
         if (active) {
-            const __half* col = base + 8 * cv;
+            const T* col = base + 8 * cv;
 #pragma unroll 4
             for (int r = row0 + rl; r < row1; r += RL) {
                 const uint4 v = *reinterpret_cast<const uint4*>(col + (long long)r * ld);
-                const __half2* h = reinterpret_cast<const __half2*>(&v);
+                const auto* h = reinterpret_cast<const typename LbType<T>::T2*>(&v);
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const float2 f = __half22float2(h[j]);
+                    const float2 f = LbType<T>::to_f2(h[j]);
                     s[2 * j] += f.x;
                     s[2 * j + 1] += f.y;
                     q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
@@ -138,11 +140,13 @@ gn_partial_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int
 }
 
 // pass 2: normalise, affine, optional SiLU.  Scale / shift of the thread's 8 channels live in registers.
+template <typename T>
 __global__ void __launch_bounds__(kThreads)
-gn_apply_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int groups,
-                const float2* __restrict__ stats, const __half* __restrict__ gamma,
-                const __half* __restrict__ beta, int do_silu, __half* __restrict__ out, long long ldo,
+gn_apply_kernel(const T* __restrict__ x, long long ld, int C, int HW, int groups,
+                const float2* __restrict__ stats, const T* __restrict__ gamma,
+                const T* __restrict__ beta, int do_silu, T* __restrict__ out, long long ldo,
                 int rows_per_block) {
+    using L = LbType<T>;
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.y;
@@ -159,33 +163,33 @@ gn_apply_kernel(const __half* __restrict__ x, long long ld, int C, int HW, int g
         {
             const uint4 gv = __ldg(reinterpret_cast<const uint4*>(gamma + 8 * cv));
             const uint4 bv = __ldg(reinterpret_cast<const uint4*>(beta + 8 * cv));
-            const __half* gh = reinterpret_cast<const __half*>(&gv);
-            const __half* bh = reinterpret_cast<const __half*>(&bv);
+            const T* gh = reinterpret_cast<const T*>(&gv);
+            const T* bh = reinterpret_cast<const T*>(&bv);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const float2 st = stats[(long long)b * groups + (8 * cv + j) / cpg];     // (mean, rstd)
-                sc[j] = st.y * __half2float(gh[j]);
-                sh[j] = __half2float(bh[j]) - st.x * sc[j];
+                sc[j] = st.y * L::to_f(gh[j]);
+                sh[j] = L::to_f(bh[j]) - st.x * sc[j];
             }
         }
-        const __half* col = x + ((long long)b * HW) * ld + 8 * cv;
-        __half* ocol = out + ((long long)b * HW) * ldo + 8 * cv;
+        const T* col = x + ((long long)b * HW) * ld + 8 * cv;
+        T* ocol = out + ((long long)b * HW) * ldo + 8 * cv;
 #pragma unroll 4
         for (int r = row0 + rl; r < row1; r += RL) {
             const uint4 v = *reinterpret_cast<const uint4*>(col + (long long)r * ld);
-            const __half2* h = reinterpret_cast<const __half2*>(&v);
+            const auto* h = reinterpret_cast<const typename L::T2*>(&v);
             uint4 o;
-            __half2* oh = reinterpret_cast<__half2*>(&o);
+            auto* oh = reinterpret_cast<typename L::T2*>(&o);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const float2 f = __half22float2(h[j]);
-                float y0 = lb_round_h(fmaf(f.x, sc[2 * j], sh[2 * j]));
-                float y1 = lb_round_h(fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]));
+                const float2 f = L::to_f2(h[j]);
+                float y0 = L::round(fmaf(f.x, sc[2 * j], sh[2 * j]));
+                float y1 = L::round(fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]));
                 if (do_silu) {
                     y0 = silu_f(y0);
                     y1 = silu_f(y1);
                 }
-                oh[j] = __floats2half2_rn(y0, y1);
+                oh[j] = L::from_f2(y0, y1);
             }
             *reinterpret_cast<uint4*>(ocol + (long long)r * ldo) = o;
         }
@@ -279,7 +283,8 @@ extern "C" size_t lb_groupnorm_workspace_bytes(lb_ctx* ctx, int B, int HW, int g
     return kGnMaxBatch * sizeof(int) + ((size_t)B * gn_chunks(HW) * groups + (size_t)B * groups) * sizeof(float2);
 }
 
-extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
+template <typename T>
+static int groupnorm_launch(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
                             const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
                             void* workspace, void* stream) {
     LB_REQUIRE(ctx && x && gamma && beta && out && workspace, "lb_groupnorm: null argument");
@@ -294,7 +299,7 @@ extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int H
     float2* stats = reinterpret_cast<float2*>(counter + kGnMaxBatch);
     float2* partial = stats + (size_t)B * groups;
     cudaStream_t st = lb_stream(stream);
-    lb_launch_pdl(gn_partial_kernel, dim3(chunks, B), kThreads, 0, st, (const __half*)x, ld, C, HW, groups, rpc, eps,
+    lb_launch_pdl(gn_partial_kernel<T>, dim3(chunks, B), kThreads, 0, st, (const T*)x, ld, C, HW, groups, rpc, eps,
                   partial, stats, counter);
     LB_LAUNCH_CHECK();
     // apply: ~6 blocks per SM over the whole batch, at least 4 rows per row lane
@@ -305,10 +310,28 @@ extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int H
     if (rpb < 4 * RL) rpb = 4 * RL;
     if (rpb > HW) rpb = HW;
     blocks = (int)lb_ceil_div(HW, rpb);
-    lb_launch_pdl(gn_apply_kernel, dim3(blocks, B), kThreads, 0, st, (const __half*)x, ld, C, HW, groups,
-                  (const float2*)stats, (const __half*)gamma, (const __half*)beta, silu, (__half*)out, ldo, rpb);
+    lb_launch_pdl(gn_apply_kernel<T>, dim3(blocks, B), kThreads, 0, st, (const T*)x, ld, C, HW, groups,
+                  (const float2*)stats, (const T*)gamma, (const T*)beta, silu, (T*)out, ldo, rpb);
     LB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int lb_groupnorm_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
+                               const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
+                               void* workspace, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_groupnorm: unknown dtype %d", dtype);
+    return dtype == LB_DTYPE_BF16
+               ? groupnorm_launch<__nv_bfloat16>(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo,
+                                                 workspace, stream)
+               : groupnorm_launch<__half>(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo, workspace,
+                                          stream);
+}
+
+extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
+                            const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
+                            void* workspace, void* stream) {
+    return lb_groupnorm_dt(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo, workspace, stream,
+                           LB_DTYPE_F16);
 }
 
 extern "C" int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C, const void* gamma,

@@ -5,6 +5,7 @@
 // turns them into prepared launches once (TMA descriptors encoded, tilings chosen) and
 // replays them on a stream with no Python, no allocation and no host sync in the loop.
 // Replaces the eager PyTorch module walk behind pipe.unet(...) (diffusers_holder.py:336-344).
+#include <stddef.h>
 #include <stdlib.h>
 
 #include <vector>
@@ -13,6 +14,8 @@
 
 // the op records are an ABI: a member may grow only inside the union's existing size (set by lb_gemm_desc)
 static_assert(sizeof(((lb_op*)nullptr)->u.resample) <= sizeof(lb_gemm_desc), "lb_op.u.resample outgrew the union");
+// lb_op.dtype took the place of a reserved int32: the record size and the union's offset are unchanged
+static_assert(sizeof(lb_op) == 8 + sizeof(lb_gemm_desc) && offsetof(lb_op, u) == 8, "lb_op layout changed");
 
 struct AttnPlan;
 int attn_plan_build_opaque(lb_ctx* ctx, const lb_attn_desc& d, void** plan_out);
@@ -59,7 +62,22 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
         nd.op = ops[i];
         nd.attn = nullptr;
         int e = 0;
-        switch (ops[i].kind) {
+        switch (ops[i].kind) {     // the kinds that have a bf16 variant; every other kind needs dtype 0
+            case LB_OP_GROUPNORM: case LB_OP_LATENT_PREP: case LB_OP_CONV_IN: case LB_OP_UPSAMPLE2X:
+            case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS:
+                if (ops[i].dtype != LB_DTYPE_F16 && ops[i].dtype != LB_DTYPE_BF16) {
+                    lb_set_error("lb_program_create: op %lld has unknown dtype %d", (long long)i, ops[i].dtype);
+                    e = 2;
+                }
+                break;
+            default:
+                if (ops[i].dtype != LB_DTYPE_F16) {
+                    lb_set_error("lb_program_create: op %lld (kind %d) has no dtype %d variant (a GEMM takes its types "
+                                 "from its mode flags)", (long long)i, ops[i].kind, ops[i].dtype);
+                    e = 2;
+                }
+        }
+        if (!e) switch (ops[i].kind) {
             case LB_OP_GEMM:
                 e = gemm_plan_build(ctx, *reinterpret_cast<const GemmDesc*>(&ops[i].u.gemm), &nd.gemm);
                 break;
@@ -188,7 +206,7 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_CONV_IN: {
                 const auto& a = o.u.conv;
-                e = lb_conv_in(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, stream);
+                e = lb_conv_in_dt(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, stream, o.dtype);
                 break;
             }
             case LB_OP_CONV_OUT: {
@@ -198,8 +216,8 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_UPSAMPLE2X: {
                 const auto& a = o.u.resample;
-                e = lb_upsample_nearest(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out,
-                                        a.Ho ? a.Ho : 2 * a.H, a.Wo ? a.Wo : 2 * a.W, stream);
+                e = lb_upsample_nearest_dt(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out,
+                                           a.Ho ? a.Ho : 2 * a.H, a.Wo ? a.Wo : 2 * a.W, stream, o.dtype);
                 break;
             }
             case LB_OP_IM2COL_S2: {
@@ -209,8 +227,8 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_GROUPNORM: {
                 const auto& a = o.u.norm;
-                e = lb_groupnorm(ctx, a.x, a.ld_x, a.B, (int)a.rows, a.C, a.groups, a.gamma, a.beta, a.eps, a.silu,
-                                 a.out, a.ld_out, a.workspace, stream);
+                e = lb_groupnorm_dt(ctx, a.x, a.ld_x, a.B, (int)a.rows, a.C, a.groups, a.gamma, a.beta, a.eps, a.silu,
+                                    a.out, a.ld_out, a.workspace, stream, o.dtype);
                 break;
             }
             case LB_OP_LAYERNORM: {
@@ -220,22 +238,22 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_LATENT_PREP: {
                 const auto& a = o.u.aux;
-                e = lb_latent_prep(ctx, a.x, a.B, a.C, a.n, a.w, a.bias, a.out, stream);
+                e = lb_latent_prep_dt(ctx, a.x, a.B, a.C, a.n, a.w, a.bias, a.out, stream, o.dtype);
                 break;
             }
             case LB_OP_SOFTMAX_ROWS: {
                 const auto& a = o.u.aux;
-                e = lb_softmax_rows(ctx, a.x, a.ld_x, a.n, a.C, a.out, a.ld_out, stream);
+                e = lb_softmax_rows_dt(ctx, a.x, a.ld_x, a.n, a.C, a.out, a.ld_out, stream, o.dtype);
                 break;
             }
             case LB_OP_POSTPROCESS_U8: {
                 const auto& a = o.u.aux;
-                e = lb_postprocess_u8(ctx, a.x, a.B, a.C, a.n, a.out, (int*)const_cast<void*>(a.w), stream);
+                e = lb_postprocess_u8_dt(ctx, a.x, a.B, a.C, a.n, a.out, (int*)const_cast<void*>(a.w), stream, o.dtype);
                 break;
             }
             case LB_OP_NHWC_TO_NCHW: {
                 const auto& a = o.u.aux;
-                e = lb_nhwc_to_nchw(ctx, a.x, a.ld_x, a.B, a.C, a.n, a.out, stream);
+                e = lb_nhwc_to_nchw_dt(ctx, a.x, a.ld_x, a.B, a.C, a.n, a.out, stream, o.dtype);
                 break;
             }
             case LB_OP_LPIPS_IM2COL_U8: {

@@ -45,7 +45,8 @@ class DiffusersHolder:
         self.width_latent = self.height_latent = s
         self.width_img = self.height_img = s * pipe.vae_scale_factor
         self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device)
-        self.vae = VAEDecoderB200(pipe.vae_state_dict, pipe.vae_channels, pipe.vae_scaling_factor, self.device)
+        self.vae = None
+        self.set_vae_dtype(getattr(pipe, "vae_dtype", "fp16"))
         self.noise_fn = None          # tests: inject the ancestral-step noise, noise_fn(i, shape)
         self.noise_fn_multi = None    # same for run_diffusion_sd_xl_multi with k > 1: noise_fn_multi(job, i, shape)
         self._cond_key = None
@@ -62,6 +63,18 @@ class DiffusersHolder:
         self._dual = {}
 
     # ---- configuration --------------------------------------------------------------------
+    def set_vae_dtype(self, vae_dtype):
+        """Rebuild the VAE decoder with "fp16" or "bf16" storage (fp32 accumulation either way).  bf16 decodes VAEs
+        whose activations overflow fp16, such as the stock SDXL VAE; a diffusers pipeline picks it from the VAE
+        config's force_upcast."""
+        from .pipe import VAE_DTYPES
+        if vae_dtype not in VAE_DTYPES:
+            raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
+        p = self.pipe
+        self.vae = VAEDecoderB200(p.vae_state_dict, p.vae_channels, p.vae_scaling_factor, self.device,
+                                  dtype=VAE_DTYPES[vae_dtype])
+        self.vae_dtype = vae_dtype
+
     def set_num_inference_steps(self, num_inference_steps):
         self.num_inference_steps = num_inference_steps
         self.pipe.scheduler.set_timesteps(num_inference_steps, device=self.device)

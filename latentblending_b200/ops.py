@@ -8,6 +8,7 @@ from . import _cabi
 from ._cabi import check, ctx, ptr, stream_ptr
 
 _DT = {torch.float16: 0, torch.float32: 1}
+_DT16 = {torch.float16: _cabi.DTYPE_F16, torch.bfloat16: _cabi.DTYPE_BF16}   # the ops with fp16 and bf16 variants
 LAUNCHES = [0]      # kernels of liblb200 launched through this module / Program.run (bench.py reports it)
 
 
@@ -113,23 +114,56 @@ def _p(t):
     return None if t is None else t.data_ptr()
 
 
+def dtype16(t, what="tensor"):
+    """LB_DTYPE_* of an fp16 / bf16 tensor; anything else raises."""
+    if t.dtype not in _DT16:
+        raise _cabi.LB200Error(f"{what} must be float16 or bfloat16 (got {t.dtype})")
+    return _DT16[t.dtype]
+
+
+def _same_dtype(dtype, what, *ts):
+    for t in ts:
+        if t is not None and t.dtype != dtype:
+            raise _cabi.LB200Error(f"{what}: mixed element types ({t.dtype} with {dtype})")
+
+
+def gemm_dtype_mode(a0, w, out_dtype, a1=None, bias=None, bias2=None, res=None):
+    """The lb_gemm mode flags of the element types: fp16 operands (0), or bf16 operands (LB_GEMM_BF16) with a bf16 or
+    (``out_dtype`` float16: LB_GEMM_OUT_F16) fp16 output.  Mixed operand types raise."""
+    if a0.dtype != torch.bfloat16 and w.dtype != torch.bfloat16:
+        return 0
+    _same_dtype(torch.bfloat16, "gemm operands a0 / w / a1 / bias / bias2 / res", a0, w, a1, bias, bias2, res)
+    if out_dtype == torch.bfloat16:
+        return _cabi.GEMM_BF16
+    if out_dtype == torch.float16:
+        return _cabi.GEMM_BF16 | _cabi.GEMM_OUT_F16
+    raise _cabi.LB200Error(f"gemm: bf16 operands give a bf16 or fp16 output (asked for {out_dtype})")
+
+
 _TILING = {"auto": 0, "box": _cabi.GEMM_TILE_BOX, "runs": _cabi.GEMM_TILE_RUNS}
 
 
 def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None, out=None,
-         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto"):
+         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto", out_dtype=None):
     """Tensor-core GEMM / implicit-GEMM conv (lb_gemm).  a0: NHWC activation viewed as
     [B*H*W, >=a0_c] (row stride = a0.stride(0)); w: [N, K] packed weights.
     ``tiling``: "auto" (the M tiling with fewer tiles), "box" (pixel boxes) or "runs" (pixel runs); all give the
-    same results."""
+    same results.
+    Element types come from the tensors: fp16 throughout, or bf16 a0 / w / a1 / bias / bias2 / res (LB_GEMM_BF16)
+    with a bf16 output, or an fp16 one when ``out_dtype`` (default: ``out``'s dtype, else a0's) is torch.float16."""
     if tiling not in _TILING:
         raise ValueError(f"tiling must be one of {sorted(_TILING)} (got {tiling!r})")
     dev = _dev(a0)
     M = B * H * W
     a0_c = a0.shape[-1] if a0_c is None else a0_c
     n_out = (N // 2 if mode == 1 else N) if out_cols is None else out_cols
+    if out_dtype is None:
+        out_dtype = out.dtype if out is not None else a0.dtype
+    elif out is not None and out.dtype != out_dtype:
+        raise _cabi.LB200Error(f"gemm: out is {out.dtype}, out_dtype {out_dtype}")
+    dmode = gemm_dtype_mode(a0, w, out_dtype, a1, bias, bias2, res)
     if out is None:
-        out = torch.empty((M, n_out), dtype=torch.float16, device=a0.device)
+        out = torch.empty((M, n_out), dtype=out_dtype, device=a0.device)
     d = _cabi.GemmDesc()
     d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(-2), a0_c
     if a1 is not None:
@@ -142,7 +176,7 @@ def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bi
     if res is not None:
         d.res, d.res_ld = _p(res), res.stride(-2)
     d.out, d.out_ld = _p(out), out.stride(-2)
-    d.mode = mode | (_cabi.GEMM_STATIC_W if static_w else 0) | (_cabi.GEMM_RELU if relu else 0) | _TILING[tiling]
+    d.mode = mode | (_cabi.GEMM_STATIC_W if static_w else 0) | (_cabi.GEMM_RELU if relu else 0) | _TILING[tiling] | dmode
     if ln is not None:
         d.ln_stats, d.ln_parts = _p(ln["stats"]), ln["stats"].shape[1]
         d.ln_csum, d.ln_bias, d.ln_eps = _p(ln["csum"]), _p(ln["bias"]), ln["eps"]
@@ -212,13 +246,16 @@ def attention(q, k, v, out, B, heads, Sq, Skv, q_col0=0, k_col0=0, v_col0=0, sca
 
 
 def groupnorm(x, B, HW, C, groups, gamma, beta, eps, silu, out=None):
+    """fp16 or bf16 (x, gamma, beta and out of one type)."""
     dev = _dev(x)
+    dt = dtype16(x, "groupnorm x")
     if out is None:
-        out = torch.empty((B * HW, C), dtype=torch.float16, device=x.device)
+        out = torch.empty((B * HW, C), dtype=x.dtype, device=x.device)
+    _same_dtype(x.dtype, "groupnorm x / gamma / beta / out", gamma, beta, out)
     lib = _cabi.load()
     ws = _gn_workspace(dev, lib.lb_groupnorm_workspace_bytes(ctx(dev), B, HW, groups))
-    check(lib.lb_groupnorm(ctx(dev), ptr(x), x.stride(0), B, HW, C, groups, ptr(gamma), ptr(beta), float(eps),
-                           int(silu), ptr(out), out.stride(0), ptr(ws), stream_ptr()), "lb_groupnorm")
+    check(lib.lb_groupnorm_dt(ctx(dev), ptr(x), x.stride(0), B, HW, C, groups, ptr(gamma), ptr(beta), float(eps),
+                              int(silu), ptr(out), out.stride(0), ptr(ws), stream_ptr(), dt), "lb_groupnorm")
     return out
 
 
@@ -255,12 +292,15 @@ def linear_small(x, w, bias=None, addend=None, act_in=0, act_out=0, out=None):
 
 
 def conv_in(x_nchw, w_packed, bias, Cout, out=None):
+    """fp16 or bf16 (x, weights, bias and out of one type)."""
     dev = _dev(x_nchw)
+    dt = dtype16(x_nchw, "conv_in x")
     B, Cin, H, W = x_nchw.shape
     if out is None:
-        out = torch.empty((B * H * W, Cout), dtype=torch.float16, device=x_nchw.device)
-    check(_cabi.load().lb_conv_in(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout, ptr(out),
-                                  out.stride(0), stream_ptr()), "lb_conv_in")
+        out = torch.empty((B * H * W, Cout), dtype=x_nchw.dtype, device=x_nchw.device)
+    _same_dtype(x_nchw.dtype, "conv_in x / w / bias / out", w_packed, bias, out)
+    check(_cabi.load().lb_conv_in_dt(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout, ptr(out),
+                                     out.stride(0), stream_ptr(), dt), "lb_conv_in")
     return out
 
 
@@ -286,10 +326,12 @@ def upsample_nearest(x, B, H, W, C, Ho, Wo, out=None):
     """F.interpolate(size=(Ho, Wo), mode="nearest") of NHWC rows [B*H*W, >=C] for Ho in {2H-1, 2H}, Wo in
     {2W-1, 2W} (lb_upsample_nearest; other sizes raise LB200Error)."""
     dev = _dev(x)
+    dt = dtype16(x, "upsample x")
     if out is None:
-        out = torch.empty((B * Ho * Wo, C), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_upsample_nearest(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), out.stride(0),
-                                           Ho, Wo, stream_ptr()), "lb_upsample_nearest")
+        out = torch.empty((B * Ho * Wo, C), dtype=x.dtype, device=x.device)
+    _same_dtype(x.dtype, "upsample x / out", out)
+    check(_cabi.load().lb_upsample_nearest_dt(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), out.stride(0),
+                                              Ho, Wo, stream_ptr(), dt), "lb_upsample_nearest")
     return out
 
 
@@ -300,4 +342,53 @@ def im2col_s2(x, B, H, W, C, out=None):
         out = torch.empty((B * Ho * Wo, 9 * C), dtype=torch.float16, device=x.device)
     check(_cabi.load().lb_im2col_s2(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), stream_ptr()),
           "lb_im2col_s2")
+    return out
+
+
+# ---- VAE-decoder helpers (fp16 or bf16; the decoder itself records them into a Program) ---------------------------
+
+
+def latent_prep(x_nchw, w_f32, bias_f32, out_dtype=torch.float16, out=None):
+    """post_quant_conv(latents / scaling_factor): fp16 NCHW latents in, ``out_dtype`` (fp16 / bf16) NCHW out."""
+    dev = _dev(x_nchw)
+    assert x_nchw.dtype == torch.float16 and x_nchw.is_contiguous()
+    B, C, H, W = x_nchw.shape
+    if out is None:
+        out = torch.empty((B, C, H, W), dtype=out_dtype, device=x_nchw.device)
+    check(_cabi.load().lb_latent_prep_dt(ctx(dev), ptr(x_nchw), B, C, H * W, ptr(w_f32), ptr(bias_f32), ptr(out),
+                                         stream_ptr(), dtype16(out, "latent_prep out")), "lb_latent_prep")
+    return out
+
+
+def softmax_rows(x, out=None, out_dtype=None):
+    """Row softmax of fp16 ``x`` [rows, cols] into fp16 or bf16 ``out`` (may be x itself)."""
+    dev = _dev(x)
+    assert x.dtype == torch.float16
+    if out is None:
+        out = torch.empty(x.shape, dtype=out_dtype or x.dtype, device=x.device)
+    check(_cabi.load().lb_softmax_rows_dt(ctx(dev), ptr(x), x.stride(0), x.shape[0], x.shape[1], ptr(out),
+                                          out.stride(0), stream_ptr(), dtype16(out, "softmax out")), "lb_softmax_rows")
+    return out
+
+
+def postprocess_u8(img_nchw, out=None, nonfinite=None):
+    """fp16 / bf16 NCHW image -> uint8 NHWC; ``nonfinite`` (device int32[1]) accumulates the non-finite pixel count."""
+    dev = _dev(img_nchw)
+    assert img_nchw.is_contiguous()
+    B, C, H, W = img_nchw.shape
+    if out is None:
+        out = torch.empty((B, H, W, C), dtype=torch.uint8, device=img_nchw.device)
+    check(_cabi.load().lb_postprocess_u8_dt(ctx(dev), ptr(img_nchw), B, C, H * W, ptr(out), ptr(nonfinite),
+                                            stream_ptr(), dtype16(img_nchw, "postprocess image")), "lb_postprocess_u8")
+    return out
+
+
+def nhwc_to_nchw(x, B, C, H, W, out=None):
+    """The first C (<= 8) columns of fp16 / bf16 NHWC rows [B*H*W, ld] -> NCHW [B, C, H, W]."""
+    dev = _dev(x)
+    if out is None:
+        out = torch.empty((B, C, H, W), dtype=x.dtype, device=x.device)
+    _same_dtype(x.dtype, "nhwc_to_nchw x / out", out)
+    check(_cabi.load().lb_nhwc_to_nchw_dt(ctx(dev), ptr(x), x.stride(0), B, C, H * W, ptr(out), stream_ptr(),
+                                          dtype16(x, "nhwc_to_nchw x")), "lb_nhwc_to_nchw")
     return out

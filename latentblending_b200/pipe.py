@@ -24,6 +24,18 @@ from .unet import UNetConfig
 SDXL_BASE = UNetConfig()
 SDXL_TURBO = UNetConfig(sample_size=64)
 VAE_CHANNELS = (128, 256, 512, 512)
+VAE_DTYPES = {"fp16": torch.float16, "bf16": torch.bfloat16}     # pipe.vae_dtype -> the VAE decoder's storage type
+
+
+def vae_dtype_from_config(vcfg):
+    """"bf16" when an AutoencoderKL config asks to be upcast (``force_upcast``, True unless the config says otherwise:
+    the diffusers default, set for the stock SDXL VAE whose activations overflow fp16), else "fp16".  The reference
+    decodes such a VAE in fp32 (diffusers_holder.py:128-139); bf16 has fp32's exponent range at the fp16 tensor rate."""
+    if isinstance(vcfg, dict):          # diffusers' FrozenDict
+        up = vcfg["force_upcast"] if "force_upcast" in vcfg else True
+    else:
+        up = getattr(vcfg, "force_upcast", True)
+    return "bf16" if up else "fp16"
 
 
 def unet_param_shapes(cfg: UNetConfig):
@@ -182,7 +194,10 @@ class SyntheticSDXLPipe:
 
     def __init__(self, name="stabilityai/stable-diffusion-xl-base-1.0", device="cuda:0", unet_cfg: UNetConfig = None,
                  seed=0, unet_state_dict=None, vae_state_dict=None, vae_channels=VAE_CHANNELS,
-                 lpips_state_dict=None):
+                 lpips_state_dict=None, vae_dtype="fp16"):
+        """``vae_dtype``: "fp16" or "bf16", the storage type of the VAE decoder DiffusersHolder builds."""
+        if vae_dtype not in VAE_DTYPES:
+            raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
         self._name_or_path = name
         self.device = torch.device(device)
         self._execution_device = self.device
@@ -196,6 +211,7 @@ class SyntheticSDXLPipe:
         self.vae_state_dict = vae_state_dict if vae_state_dict is not None else \
             random_state_dict(vae_param_shapes(vae_channels), seed + 1, self.device, damp=0.3)
         self.vae_scaling_factor = 0.13025
+        self.vae_dtype = vae_dtype
         self.lpips_state_dict = lpips_state_dict
         self.h2d_bytes = 0        # bytes of conditioning copied host->device (bench e2e)
 
@@ -232,6 +248,8 @@ class DiffusersSDXLPipe:
     are the ones the packers use), the UNet config, the scheduler config (EulerTables), ``encode_prompt`` (the CLIP text
     encoders stay PyTorch modules: they run once per prompt and are outside the hot path, SURVEY section 8f #4) and
     ``_execution_device`` / ``_name_or_path`` / ``default_sample_size`` / ``vae_scale_factor``.
+    ``vae_dtype`` follows the VAE config: "bf16" when it sets ``force_upcast`` (the stock SDXL VAE, where the reference
+    decodes in fp32), "fp16" for an fp16-safe VAE that turns it off.
     ``lpips_state_dict`` must be supplied (see INTEGRATION.md "LPIPS weights"): with real weights a random LPIPS
     network would silently steer the branch placement."""
     is_synthetic = False
@@ -277,6 +295,7 @@ class DiffusersSDXLPipe:
         vcfg = pipe.vae.config
         self.vae_channels = tuple(vcfg["block_out_channels"] if "block_out_channels" in vcfg else vcfg.block_out_channels)
         self.vae_scaling_factor = float(vcfg["scaling_factor"] if "scaling_factor" in vcfg else vcfg.scaling_factor)
+        self.vae_dtype = vae_dtype_from_config(vcfg)
         self.lpips_state_dict = lpips_state_dict if lpips_state_dict is not None else getattr(pipe, "lpips_state_dict", None)
         self.h2d_bytes = 0
 

@@ -87,7 +87,10 @@ class Program:
         is used as the B operand.
         ``ln``: dict(stats=[M,parts,2] fp32, csum=[N] fp32, bias=[N] fp32, eps) -- LayerNorm folded into this GEMM
         (``w`` must already hold w*gamma; see include/lb200.h).  ``stats_out``: [M,parts,2] fp32 buffer that receives
-        this GEMM's per-row partial sums for a following LN-folded GEMM (parts = self.gemm_stats_parts(...))."""
+        this GEMM's per-row partial sums for a following LN-folded GEMM (parts = self.gemm_stats_parts(...)).
+        Element types come from the tensors as in ``ops.gemm``: bf16 operands (LB_GEMM_BF16) write ``out``'s type."""
+        from .ops import gemm_dtype_mode
+        dmode = gemm_dtype_mode(a0, w, out.dtype, a1, bias, bias2, res)
         d = self._new(OP_GEMM).u.gemm
         d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(0), (a0.shape[1] if a0_c is None else a0_c)
         if a1 is not None:
@@ -100,7 +103,7 @@ class Program:
         if res is not None:
             d.res, d.res_ld = _p(res), res.stride(0)
         d.out, d.out_ld = _p(out), out.stride(0)
-        d.mode = mode | (GEMM_STATIC_W if static_w else 0) | (GEMM_RELU if relu else 0)
+        d.mode = mode | (GEMM_STATIC_W if static_w else 0) | (GEMM_RELU if relu else 0) | dmode
         if ln is not None:
             st = ln["stats"]
             assert st.dtype == torch.float32 and st.dim() == 3 and st.shape[2] == 2 and st.is_contiguous()
@@ -150,8 +153,15 @@ class Program:
         d.B, d.heads, d.Sq, d.Skv, d.head_dim, d.scale = B, heads, Sq, Skv, 64, scale
         self.hold(q, k, v, out)
 
-    def groupnorm(self, x, B, HW, C, groups, gamma, beta, eps, silu, out, ws):
-        d = self._new(OP_GROUPNORM).u.norm
+    # The VAE-decoder builders below take ``dtype`` (LB_DTYPE_F16 = 0 / LB_DTYPE_BF16 = 1): the lb_op.dtype of the
+    # record, i.e. the element type of their 16-bit tensors (see include/lb200.h for each op's meaning).
+    def _new_dt(self, kind, dtype):
+        op = self._new(kind)
+        op.dtype = dtype
+        return op
+
+    def groupnorm(self, x, B, HW, C, groups, gamma, beta, eps, silu, out, ws, dtype=0):
+        d = self._new_dt(OP_GROUPNORM, dtype).u.norm
         d.x, d.ld_x, d.rows, d.B, d.C, d.groups, d.silu, d.eps = _p(x), x.stride(0), HW, B, C, groups, int(silu), eps
         d.gamma, d.beta, d.out, d.ld_out, d.workspace = _p(gamma), _p(beta), _p(out), out.stride(0), _p(ws)
         self.hold(x, gamma, beta, out, ws)
@@ -178,8 +188,8 @@ class Program:
         d.act_in, d.act_out, d.out, d.ldo, d.N = act_in, act_out, _p(out), out.stride(0), w.shape[0]
         self.hold(x, w, out, bias, addend)
 
-    def conv_in(self, x_nchw, w, bias, Cout, out):
-        d = self._new(OP_CONV_IN).u.conv
+    def conv_in(self, x_nchw, w, bias, Cout, out, dtype=0):
+        d = self._new_dt(OP_CONV_IN, dtype).u.conv
         B, Cin, H, W = x_nchw.shape
         d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
         d.out, d.ld_out = _p(out), out.stride(0)
@@ -191,17 +201,17 @@ class Program:
         d.w, d.bias, d.Cout, d.out = _p(w), _p(bias), Cout, _p(out_nchw)
         self.hold(x, w, bias, out_nchw)
 
-    def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp):
+    def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp, dtype=0):
         """The C0 -> Cout (<= 8) 3x3 output convolution on the tensor-core GEMM: N = 8 (zero-padded weight rows),
-        then the Cout live columns go back to NCHW.  ``tmp``: [B*H*W, 8] fp16 scratch."""
+        then the Cout live columns go back to NCHW.  ``tmp``: [B*H*W, 8] scratch of the decoder's type."""
         self.gemm(x, w8, 8, B, H, W, tmp, taps=9, a0_c=Cin, bias=bias8)
-        d = self._new(OP_NHWC_TO_NCHW).u.aux
+        d = self._new_dt(OP_NHWC_TO_NCHW, dtype).u.aux
         d.x, d.ld_x, d.out, d.n, d.B, d.C = _p(tmp), tmp.stride(0), _p(out_nchw), H * W, B, Cout
         self.hold(tmp, out_nchw)
 
-    def upsample2x(self, x, B, H, W, C, out, Ho=0, Wo=0):
+    def upsample2x(self, x, B, H, W, C, out, Ho=0, Wo=0, dtype=0):
         """Nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}; 0 = exactly 2x)."""
-        d = self._new(OP_UPSAMPLE2X).u.resample
+        d = self._new_dt(OP_UPSAMPLE2X, dtype).u.resample
         d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
         d.Ho, d.Wo = Ho, Wo
         self.hold(x, out)
@@ -211,19 +221,20 @@ class Program:
         d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
         self.hold(x, out)
 
-    def latent_prep(self, x_nchw, w_f32, bias_f32, out_nchw):
-        d = self._new(OP_LATENT_PREP).u.aux
+    def latent_prep(self, x_nchw, w_f32, bias_f32, out_nchw, dtype=0):
+        d = self._new_dt(OP_LATENT_PREP, dtype).u.aux
         B, C, H, W = x_nchw.shape
         d.x, d.w, d.bias, d.out, d.n, d.B, d.C = _p(x_nchw), _p(w_f32), _p(bias_f32), _p(out_nchw), H * W, B, C
         self.hold(x_nchw, w_f32, bias_f32, out_nchw)
 
-    def softmax_rows(self, x, out):
-        d = self._new(OP_SOFTMAX_ROWS).u.aux
+    def softmax_rows(self, x, out, dtype=0):
+        """fp16 rows in; ``dtype``: the output's type (may write over ``x``, see lb_softmax_rows_dt)."""
+        d = self._new_dt(OP_SOFTMAX_ROWS, dtype).u.aux
         d.x, d.ld_x, d.out, d.ld_out, d.n, d.C = _p(x), x.stride(0), _p(out), out.stride(0), x.shape[0], x.shape[1]
         self.hold(x, out)
 
-    def postprocess_u8(self, img_nchw, out_u8, nonfinite=None):
-        d = self._new(OP_POSTPROCESS_U8).u.aux
+    def postprocess_u8(self, img_nchw, out_u8, nonfinite=None, dtype=0):
+        d = self._new_dt(OP_POSTPROCESS_U8, dtype).u.aux
         B, C, H, W = img_nchw.shape
         d.x, d.out, d.n, d.B, d.C, d.w = _p(img_nchw), _p(out_u8), H * W, B, C, _p(nonfinite)
         self.hold(img_nchw, out_u8, nonfinite)
@@ -285,9 +296,9 @@ def pack_conv_out8(w_co_ky_kx_ci, bias):
     co, cin = w_co_ky_kx_ci.shape[0], w_co_ky_kx_ci.shape[-1]
     if cin % 64 != 0 or co > 8:
         return None, None
-    w8 = torch.zeros(8, 9 * cin, dtype=torch.float16, device=w_co_ky_kx_ci.device)
+    w8 = torch.zeros(8, 9 * cin, dtype=w_co_ky_kx_ci.dtype, device=w_co_ky_kx_ci.device)     # fp16, or bf16
     w8[:co] = w_co_ky_kx_ci.reshape(co, 9 * cin)
-    b8 = torch.zeros(8, dtype=torch.float16, device=bias.device)
+    b8 = torch.zeros(8, dtype=bias.dtype, device=bias.device)
     b8[:co] = bias
     return w8.contiguous(), b8.contiguous()
 
