@@ -140,7 +140,7 @@ typedef struct lb_gemm_desc {
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
     int32_t mode;     /* low byte: 0 = linear epilogue, 1 = GEGLU; flags: LB_GEMM_STATIC_W, LB_GEMM_RELU,
-                         LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS, LB_GEMM_BF16, LB_GEMM_OUT_F16 */
+                         LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS, LB_GEMM_BF16, LB_GEMM_OUT_F16, LB_GEMM_D2S2 */
     const void* ln_stats; int32_t ln_parts;      /* float2 [M][ln_parts] or NULL */
     const void* ln_csum; const void* ln_bias;    /* float [N] each */
     float ln_eps;
@@ -162,6 +162,15 @@ typedef struct lb_gemm_desc {
 /* mode flag, only with LB_GEMM_BF16: bf16 operands, fp16 output (the VAE attention scores, whose fp16 rounding is 8x
  * finer than bf16's and whose magnitudes stay far inside fp16's range; lb_softmax_rows_dt reads them as fp16) */
 #define LB_GEMM_OUT_F16 0x2000
+/* mode flag: nearest-2x upsample followed by a 3x3 conv as ONE GEMM over the low-resolution map (the upsampling
+ * convolutions of the tiny VAE decoder, AutoencoderTiny).  taps = 9 over a B x H x W map a0 with N = 4 * Co: the weight
+ * rows are four phase filters, row p * Co + c with p = 2a + b, each a 3x3 filter over LOW-resolution taps (the original
+ * filter's taps summed onto the low-resolution pixel they read after upsampling; see latentblending_b200/taesd.py).
+ * Accumulator column p * Co + c of low-resolution pixel (img, y, x) is stored at output pixel (img, 2y + a, 2x + b),
+ * channel c, of the NHWC output [4*B*H*W rows, row stride out_ld]: the upsampled input is never materialised.
+ * fp16, linear epilogue (+ bias[N], LB_GEMM_RELU); rejected with res, bias2, a1, the LayerNorm fold, stats_out,
+ * GEGLU or LB_GEMM_BF16, with taps != 9 and with N % 32 != 0 (so Co % 8 == 0). */
+#define LB_GEMM_D2S2 0x4000
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
 /* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
  * that holds a row of the wgmma accumulator); < 0 on error */
@@ -247,6 +256,17 @@ int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W,
                   const void* bias, int Cout, void* out, int64_t ldo, void* stream, int dtype);
 int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
                            int64_t ldo, int Ho, int Wo, void* stream, int dtype);
+/* lb_conv_in_act: lb_conv_in_dt with an input transform and an output activation chosen by ``act``:
+ *   act 0: lb_conv_in_dt itself (in_scale unused);
+ *   act 1: the tiny VAE decoder's input stage (AutoencoderTiny: decoder(latents / scaling_factor), whose first
+ *          steps are tanh(z / 3) * 3, Conv2d(4, C, 3, padding=1), ReLU).  Each input v becomes
+ *          h(h(tanh(h(h(v * in_scale) / 3))) * 3), h = rounding to fp16 (the fp16 roundings of the reference's
+ *          ``/ scaling_factor``, ``/ 3``, ``tanh`` and ``* 3``; in_scale = 1 / scaling_factor), then the 3x3 conv +
+ *          bias, then max(., 0).  fp16 only (dtype LB_DTYPE_F16).
+ * Same layouts and limits as lb_conv_in. */
+int lb_conv_in_act(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                   const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream,
+                   int dtype);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
 
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
@@ -320,15 +340,17 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * lb_program_run replays it on ``stream`` (``t`` = the timestep fed to
  * LB_OP_EMBED_INPUTS).  Replaces the module walk of pipe.unet(...)
  * (diffusers_holder.py:336-344).
- * lb_op.dtype: the element type (LB_DTYPE_*) of GROUPNORM, LATENT_PREP, CONV_IN, UPSAMPLE2X, NHWC_TO_NCHW,
- * POSTPROCESS_U8 and SOFTMAX_ROWS (for SOFTMAX_ROWS the output's: see lb_softmax_rows_dt), i.e. which ``*_dt`` call
- * the record makes.  It must be 0 for every other kind (a GEMM takes its types from its mode flags).
+ * lb_op.dtype: the element type (LB_DTYPE_*) of GROUPNORM, LATENT_PREP, CONV_IN, CONV_IN_ACT, UPSAMPLE2X,
+ * NHWC_TO_NCHW, POSTPROCESS_U8 and SOFTMAX_ROWS (for SOFTMAX_ROWS the output's: see lb_softmax_rows_dt), i.e. which
+ * ``*_dt`` call the record makes.  It must be 0 for every other kind (a GEMM takes its types from its mode flags).
+ * LB_OP_CONV_IN_ACT: lb_conv_in_act (record u.conv_act).
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
     LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_CONV_OUT = 8, LB_OP_UPSAMPLE2X = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
-    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17
+    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17,
+    LB_OP_CONV_IN_ACT = 18
 };
 typedef struct lb_op {
     int32_t kind;
@@ -345,6 +367,9 @@ typedef struct lb_op {
                  const void* addend; int64_t ldadd; int32_t act_in, act_out; void* out; int64_t ldo; int32_t N; } lin;
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
                  int32_t Cout; void* out; int64_t ld_out; } conv;
+        /* CONV_IN_ACT: the CONV_IN fields, then lb_conv_in_act's act and in_scale */
+        struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
+                 int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale; } conv_act;
         /* UPSAMPLE2X: output Ho x Wo (0 = 2H / 2W; see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
         struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; int32_t Ho, Wo; } resample;
         /* LATENT_PREP: x,w,bias,out,B,C,n=h*w; SOFTMAX_ROWS: x,ld_x,out,ld_out,n=rows,C=cols;

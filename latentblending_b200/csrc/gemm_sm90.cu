@@ -39,6 +39,10 @@
 // template parameter that changes only the TMA element type, the wgmma input type and the epilogue's loads / stores
 // (bf16 kernels: linear epilogue only; LB_GEMM_OUT_F16 stores fp16).  Both are 2 bytes, so boxes, swizzle, ring and
 // tilings are shared.
+// Depth-to-space (LB_GEMM_D2S2, gemm_tc_d2s_kernel): nearest-2x upsample + 3x3 conv as one GEMM over the
+// low-resolution map -- N = 4 * Co phase filters, and the linear epilogue stores column p * Co + c of pixel (y, x) at
+// upsampled pixel (2y + a, 2x + b), p = 2a + b (the tiny VAE decoder's upsampling convolutions).  The existing kernels
+// instantiate the same body with the store off.
 // Bound: tensor pipe; algorithmic FLOPs = 2*M*N*K.
 #include "gemm_sm90.cuh"
 #include <stdlib.h>
@@ -133,12 +137,17 @@ struct EpiRow {
 // the order is safe, and the loads overlap instead of costing one L2 round trip per 8-column group.
 // T: the element type of bias, bias2, res and out (bf16 kernels store fp16 instead when p.out_f16 is set); the
 // LayerNorm fold and stats_out exist in the fp16 kernels only.
-template <int BN, typename T>
+// kD2S (LB_GEMM_D2S2, fp16 only): depth-to-space store.  Row r is low-resolution pixel (b, y, x) of a B x H x W map and
+// column n = ph * Co + c (Co = p.d2s_co, ph = 2a + b') goes to output pixel (b, 2y + a, 2x + b'), channel c, of the
+// B x 2H x 2W NHWC output.  Co % 8 == 0, so an 8-column group never straddles two phases; the phase of each group is
+// tracked incrementally across the unrolled group loop (one division per row, none per group).
+template <int BN, typename T, bool kD2S = false>
 __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float (&acc)[BN / 2], const EpiRow (&r)[2],
                                                 int n_tile, int quad) {
     using L = LbType<T>;
     using T2 = typename L::T2;
     constexpr bool kF16 = std::is_same<T, __half>::value;
+    static_assert(!kD2S || kF16, "the depth-to-space epilogue is fp16-only");
     constexpr int G = BN / 8;                    // 8-column groups per row
     constexpr int CH = G > 10 ? G / 2 : G;       // groups per load batch (register budget)
     static_assert(G % CH == 0, "load batches must tile the row");
@@ -147,9 +156,25 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
     for (int i = 0; i < 2; ++i) {
         if (!r[i].ok) continue;
         float st_sum = 0.f, st_sq = 0.f;
-        const T* res_row = p.res ? reinterpret_cast<const T*>(p.res) + r[i].row * p.ldr : nullptr;
-        const T* b2_row = p.bias2 ? reinterpret_cast<const T*>(p.bias2) + (long long)r[i].bidx * p.bias2_ld : nullptr;
+        // (no residual, bias2, LayerNorm fold or stats_out with depth-to-space: rejected on the host)
+        const T* res_row = (!kD2S && p.res) ? reinterpret_cast<const T*>(p.res) + r[i].row * p.ldr : nullptr;
+        const T* b2_row =
+            (!kD2S && p.bias2) ? reinterpret_cast<const T*>(p.bias2) + (long long)r[i].bidx * p.bias2_ld : nullptr;
         T* out_row = reinterpret_cast<T*>(p.out) + r[i].row * p.ldo;
+        // depth-to-space: ph / cc are the phase and channel of the current group's first column (n_base - 2 quad);
+        // d2s_px is the output row of phase 0 (b, 2y, 2x), d2s_row2 the row distance of phase a = 1 (one output row)
+        int ph = 0, cc = 0;
+        long long d2s_px = 0, d2s_row2 = 0;
+        if constexpr (kD2S) {
+            const int col0 = n_tile * BN;
+            ph = col0 / p.d2s_co;
+            cc = col0 - ph * p.d2s_co;
+            const int W = p.W, HW = p.H * p.W;
+            const int b = (int)(r[i].row / HW), rem = (int)(r[i].row - (long long)b * HW);
+            const int y = rem / W, x = rem - y * W;
+            d2s_row2 = 2LL * W;
+            d2s_px = ((long long)b * 2 * p.H + 2 * y) * d2s_row2 + 2 * x;
+        }
 #pragma unroll
         for (int c0 = 0; c0 < G; c0 += CH) {
             float v[CH][2];
@@ -158,7 +183,7 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                 v[g][0] = acc[4 * (c0 + g) + 2 * i];
                 v[g][1] = acc[4 * (c0 + g) + 2 * i + 1];
             }
-            if (kF16 && p.ln_stats) {
+            if (!kD2S && kF16 && p.ln_stats) {
                 constexpr int CL = CH > 8 ? CH / 2 : CH;     // fp32 vectors: half the batch
 #pragma unroll
                 for (int l0 = 0; l0 < CH; l0 += CL) {
@@ -214,7 +239,11 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                         v0 = fmaxf(v0, 0.f);
                         v1 = fmaxf(v1, 0.f);
                     }
-                    if constexpr (kF16) {
+                    if constexpr (kD2S) {
+                        const long long orow = d2s_px + (ph >> 1) * d2s_row2 + (ph & 1);
+                        *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + orow * p.ldo + cc + 2 * quad) =
+                            __floats2half2_rn(v0, v1);
+                    } else if constexpr (kF16) {
                         const __half2 o = __floats2half2_rn(v0, v1);
                         *reinterpret_cast<__half2*>(out_row + n) = o;
                         if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
@@ -228,9 +257,13 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                         *reinterpret_cast<T2*>(out_row + n) = L::from_f2(v0, v1);
                     }
                 }
+                if constexpr (kD2S) {
+                    cc += 8;
+                    if (cc == p.d2s_co) { cc = 0; ++ph; }
+                }
             }
         }
-        if (kF16 && p.stats_out)
+        if (!kD2S && kF16 && p.stats_out)
             p.stats_out[r[i].row * (kEpiParts * p.tiles_n) + kEpiParts * n_tile + quad] = make_float2(st_sum, st_sq);
     }
 }
@@ -291,8 +324,9 @@ __device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float 
 
 // kRuns: pixel-run M tiles (p.runs = 1); a separate instantiation, so the pixel-box kernels stay as they were.
 // T: operand / epilogue element type, __half or __nv_bfloat16 (LB_GEMM_BF16; linear epilogue only).
-template <int BN, bool kRuns, typename T>
-__global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+// kD2S: the depth-to-space store of LB_GEMM_D2S2 (its own kernels, gemm_tc_d2s_kernel, below).
+template <int BN, bool kRuns, typename T, bool kD2S>
+__device__ __forceinline__ void gemm_tc_body(const GemmParams& p) {
     using C = Cfg<BN>;
     constexpr bool kF16 = std::is_same<T, __half>::value;
     constexpr int nst = C::stages;
@@ -522,10 +556,21 @@ __global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
         for (int hh = 0; hh < kHalves; ++hh) {
             if constexpr (kRuns) rows_of_half(hh);
-            if (p.mode == 0) epilogue_linear<BN, T>(p, acc[hh], er[hh], n_tile, quad);
-            else if constexpr (kF16 && BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
+            if (p.mode == 0) epilogue_linear<BN, T, kD2S>(p, acc[hh], er[hh], n_tile, quad);
+            else if constexpr (!kD2S && kF16 && BN == kGegluBN) epilogue_geglu<BN>(p, acc[hh], er[hh], n_tile, quad);
         }
     }
+}
+
+template <int BN, bool kRuns, typename T>
+__global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+    gemm_tc_body<BN, kRuns, T, false>(p);
+}
+
+// LB_GEMM_D2S2: nearest-2x upsample + 3x3 conv as one GEMM over the low-resolution map (fp16)
+template <int BN, bool kRuns>
+__global__ void __launch_bounds__(kThreadsGemm, 1) gemm_tc_d2s_kernel(const __grid_constant__ GemmParams p) {
+    gemm_tc_body<BN, kRuns, __half, true>(p);
 }
 
 // ---- host side ------------------------------------------------------------------------
@@ -646,23 +691,24 @@ const char* box_tiling(const GemmDesc& d, int* tw, int* th, int* tb) {
     return nullptr;
 }
 
-template <int BN, bool kRuns, typename T> int launch_tiled(const GemmPlan& plan, cudaStream_t st) {
+template <int BN, bool kRuns, typename T, bool kD2S> int launch_tiled(const GemmPlan& plan, cudaStream_t st) {
+    void (*const kernel)(const GemmParams) = kD2S ? gemm_tc_d2s_kernel<BN, kRuns> : gemm_tc_kernel<BN, kRuns, T>;
     static bool attr_set = false;
     if (!attr_set) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, kRuns, T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           Cfg<BN>::smem_bytes));
+        LB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::smem_bytes));
         attr_set = true;
     }
-    LB_CHECK_CUDA(lb_launch_pdl(gemm_tc_kernel<BN, kRuns, T>, dim3((unsigned)plan.grid), dim3(kThreadsGemm),
-                                (size_t)Cfg<BN>::smem_bytes, st, plan.p));
+    LB_CHECK_CUDA(lb_launch_pdl(kernel, dim3((unsigned)plan.grid), dim3(kThreadsGemm), (size_t)Cfg<BN>::smem_bytes, st,
+                                plan.p));
     return 0;
 }
 
-template <int BN, typename T> int launch_bn_t(const GemmPlan& plan, cudaStream_t st) {
-    return plan.p.runs ? launch_tiled<BN, true, T>(plan, st) : launch_tiled<BN, false, T>(plan, st);
+template <int BN, typename T, bool kD2S = false> int launch_bn_t(const GemmPlan& plan, cudaStream_t st) {
+    return plan.p.runs ? launch_tiled<BN, true, T, kD2S>(plan, st) : launch_tiled<BN, false, T, kD2S>(plan, st);
 }
 
 template <int BN> int launch_bn(const GemmPlan& plan, cudaStream_t st) {
+    if (plan.d2s) return launch_bn_t<BN, __half, true>(plan, st);
     return plan.bf16 ? launch_bn_t<BN, __nv_bfloat16>(plan, st) : launch_bn_t<BN, __half>(plan, st);
 }
 
@@ -683,9 +729,20 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     GemmParams& p = plan->p;
     memset(&p, 0, sizeof(p));
     LB_REQUIRE((d.mode & ~(0xff | LB_GEMM_STATIC_W | LB_GEMM_RELU | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 |
-                           LB_GEMM_OUT_F16)) == 0,
+                           LB_GEMM_OUT_F16 | LB_GEMM_D2S2)) == 0,
                "gemm: unknown mode flags 0x%x", d.mode);
     const bool bf16 = (d.mode & LB_GEMM_BF16) != 0;
+    const bool d2s = (d.mode & LB_GEMM_D2S2) != 0;
+    if (d2s) {
+        LB_REQUIRE(d.taps == 9, "gemm: LB_GEMM_D2S2 needs a 3x3 convolution (taps = 9, got %d)", d.taps);
+        LB_REQUIRE(d.N % 32 == 0, "gemm: LB_GEMM_D2S2 needs N %% 32 == 0 (4 phases x a multiple of 8 channels; got %d)",
+                   d.N);
+        LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_D2S2 supports the linear epilogue only (no GEGLU)");
+        LB_REQUIRE(!bf16, "gemm: LB_GEMM_D2S2 is fp16-only (no LB_GEMM_BF16)");
+        LB_REQUIRE(!d.res && !d.bias2 && !d.a1, "gemm: LB_GEMM_D2S2 takes no residual, bias2 or second input");
+        LB_REQUIRE(!d.ln_stats && !d.stats_out, "gemm: LB_GEMM_D2S2 does not support the LayerNorm fold or stats_out");
+    }
+    plan->d2s = d2s;
     LB_REQUIRE(bf16 || !(d.mode & LB_GEMM_OUT_F16), "gemm: LB_GEMM_OUT_F16 needs LB_GEMM_BF16");
     if (bf16) {
         LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_BF16 supports the linear epilogue only (no GEGLU)");
@@ -781,6 +838,7 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     p.out = static_cast<__half*>(d.out);
     p.ldo = d.out_ld;
     p.out_f16 = (d.mode & LB_GEMM_OUT_F16) ? 1 : 0;
+    p.d2s_co = d2s ? d.N / 4 : 0;
     p.bias = static_cast<const __half*>(d.bias);
     p.bias2 = static_cast<const __half*>(d.bias2);
     p.bias2_ld = d.bias2_ld;

@@ -15,7 +15,7 @@ struct GemmDesc {
     const void* res; int64_t res_ld;
     void* out; int64_t out_ld;
     int32_t mode;   // low byte: 0 linear epilogue, 1 GEGLU (N accumulators -> N/2 outputs); | LB_GEMM_STATIC_W | LB_GEMM_RELU
-                    // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 | LB_GEMM_OUT_F16
+                    // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 | LB_GEMM_OUT_F16 | LB_GEMM_D2S2
     // LayerNorm folded into this GEMM (see include/lb200.h)
     const void* ln_stats; int32_t ln_parts;
     const void* ln_csum; const void* ln_bias; float ln_eps;
@@ -53,12 +53,14 @@ struct alignas(64) GemmParams {
     int runs;
     int M, HW;
     int out_f16;   // bf16 instantiations: the output is stored as fp16 (LB_GEMM_OUT_F16)
+    int d2s_co;    // depth-to-space kernels (LB_GEMM_D2S2): output channels per phase, N / 4
 };
 
 struct GemmPlan {
     GemmParams p;
     int bn;        // N tile: 64 / 128 / 160 / 256
     bool bf16;     // operands, bias, residual (and, unless p.out_f16, the output) are bf16
+    bool d2s;      // LB_GEMM_D2S2: the depth-to-space kernels
     int grid;
 };
 

@@ -110,10 +110,17 @@ linear_small_kernel(const __half* __restrict__ x, long long ldx, int M, int K, c
 
 // ---- conv_in: NCHW [B,Cin<=8,H,W] -> NHWC [B*H*W, Cout], 3x3 pad 1 -------------------------------
 // weights packed [ky][kx][cin][Cout] fp16 (bf16 in the bf16 variant) so a lane reads 8 consecutive output channels.
-template <typename T>
-__global__ void __launch_bounds__(kThreads)
-conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* __restrict__ wp,
-               const T* __restrict__ bias, int Cout, T* __restrict__ out, long long ldo) {
+// kTiny (lb_conv_in_act act 1, fp16): the tiny VAE decoder's input stage -- every input v is clamped to
+// h(h(tanh(h(h(v * in_scale) / 3))) * 3) (h: fp16 rounding, at the reference's points), and ReLU follows the conv.
+__device__ __forceinline__ float tiny_vae_input(float v, float in_scale) {
+    const float z = lb_round_h(v * in_scale);
+    return lb_round_h(lb_round_h(tanhf(lb_round_h(z / 3.0f))) * 3.0f);
+}
+
+template <typename T, bool kTiny>
+__device__ __forceinline__ void conv_in_body(const T* __restrict__ x, int B, int Cin, int H, int W,
+                                             const T* __restrict__ wp, const T* __restrict__ bias, int Cout,
+                                             T* __restrict__ out, long long ldo, float in_scale) {
     using L = LbType<T>;
     pdl_launch_dependents();
     pdl_wait();
@@ -147,7 +154,8 @@ conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* _
                     const int xx = xw + kx - 1;
                     if (xx < 0 || xx >= W) continue;
                     for (int c = 0; c < Cin; ++c) {
-                        const float xv = L::to_f(x[(((long long)b * Cin + c) * H + yy) * W + xx]);
+                        float xv = L::to_f(x[(((long long)b * Cin + c) * H + yy) * W + xx]);
+                        if constexpr (kTiny) xv = tiny_vae_input(xv, in_scale);
                         const uint4 wv = *reinterpret_cast<const uint4*>(s_w + ((ky * 3 + kx) * Cin + c) * Cout + g * 8);
                         const auto* wh = reinterpret_cast<const typename L::T2*>(&wv);
 #pragma unroll
@@ -159,6 +167,10 @@ conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* _
                     }
                 }
             }
+            if constexpr (kTiny) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) acc[j] = fmaxf(acc[j], 0.f);
+            }
             uint4 o;
             auto* oh = reinterpret_cast<typename L::T2*>(&o);
 #pragma unroll
@@ -166,6 +178,19 @@ conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* _
             *reinterpret_cast<uint4*>(out + pix * ldo + g * 8) = o;
         }
     }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+conv_in_kernel(const T* __restrict__ x, int B, int Cin, int H, int W, const T* __restrict__ wp,
+               const T* __restrict__ bias, int Cout, T* __restrict__ out, long long ldo) {
+    conv_in_body<T, false>(x, B, Cin, H, W, wp, bias, Cout, out, ldo, 1.0f);
+}
+
+__global__ void __launch_bounds__(kThreads)
+conv_in_tiny_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const __half* __restrict__ wp,
+                    const __half* __restrict__ bias, int Cout, __half* __restrict__ out, long long ldo, float in_scale) {
+    conv_in_body<__half, true>(x, B, Cin, H, W, wp, bias, Cout, out, ldo, in_scale);
 }
 
 // ---- conv_out: NHWC [B*H*W, Cin] -> NCHW [B,Cout<=4,H,W], 3x3 pad 1; one warp per pixel -----------
@@ -350,6 +375,31 @@ extern "C" int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, in
 extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
                           const void* bias, int Cout, void* out, int64_t ldo, void* stream) {
     return lb_conv_in_dt(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream, LB_DTYPE_F16);
+}
+
+extern "C" int lb_conv_in_act(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                              const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream,
+                              int dtype) {
+    LB_REQUIRE(act == 0 || act == 1, "lb_conv_in_act: unknown act %d (0 = plain, 1 = tiny VAE input stage)", act);
+    if (act == 0) return lb_conv_in_dt(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream, dtype);
+    LB_REQUIRE(dtype == LB_DTYPE_F16, "lb_conv_in_act: the tiny VAE input stage (act 1) is fp16-only (dtype %d)", dtype);
+    LB_REQUIRE(ctx && x_nchw && w_packed && bias && out, "lb_conv_in_act: null argument");
+    LB_REQUIRE(Cin >= 1 && Cin <= 8 && Cout % 8 == 0 && ldo % 8 == 0, "lb_conv_in_act: Cin<=8, Cout%%8==0 required");
+    LB_REQUIRE(isfinite(in_scale), "lb_conv_in_act: in_scale must be finite");
+    const int smem = 9 * Cin * Cout * 2;
+    LB_REQUIRE(smem <= 96 * 1024, "lb_conv_in_act: weights do not fit shared memory");
+    static bool attr = false;
+    if (!attr) {
+        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_in_tiny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        attr = true;
+    }
+    const long long npix = (long long)B * H * W;
+    unsigned grid = (unsigned)lb_ceil_div(npix, kThreads / 32);
+    if (grid > (unsigned)ctx->sm_count * 4) grid = ctx->sm_count * 4;
+    lb_launch_pdl(conv_in_tiny_kernel, grid, kThreads, smem, lb_stream(stream), (const __half*)x_nchw, B, Cin, H, W,
+                  (const __half*)w_packed, (const __half*)bias, Cout, (__half*)out, (long long)ldo, in_scale);
+    LB_LAUNCH_CHECK();
+    return 0;
 }
 
 extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,

@@ -14,6 +14,7 @@
 
 // the op records are an ABI: a member may grow only inside the union's existing size (set by lb_gemm_desc)
 static_assert(sizeof(((lb_op*)nullptr)->u.resample) <= sizeof(lb_gemm_desc), "lb_op.u.resample outgrew the union");
+static_assert(sizeof(((lb_op*)nullptr)->u.conv_act) <= sizeof(lb_gemm_desc), "lb_op.u.conv_act outgrew the union");
 // lb_op.dtype took the place of a reserved int32: the record size and the union's offset are unchanged
 static_assert(sizeof(lb_op) == 8 + sizeof(lb_gemm_desc) && offsetof(lb_op, u) == 8, "lb_op layout changed");
 
@@ -64,7 +65,7 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
         int e = 0;
         switch (ops[i].kind) {     // the kinds that have a bf16 variant; every other kind needs dtype 0
             case LB_OP_GROUPNORM: case LB_OP_LATENT_PREP: case LB_OP_CONV_IN: case LB_OP_UPSAMPLE2X:
-            case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS:
+            case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS: case LB_OP_CONV_IN_ACT:
                 if (ops[i].dtype != LB_DTYPE_F16 && ops[i].dtype != LB_DTYPE_BF16) {
                     lb_set_error("lb_program_create: op %lld has unknown dtype %d", (long long)i, ops[i].dtype);
                     e = 2;
@@ -89,6 +90,17 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
                 break;
+            case LB_OP_CONV_IN_ACT: {
+                const auto& a = ops[i].u.conv_act;
+                if (a.act != 0 && a.act != 1) {
+                    lb_set_error("lb_program_create: op %lld: unknown conv_in act %d", (long long)i, a.act);
+                    e = 2;
+                } else if (a.act == 1 && ops[i].dtype != LB_DTYPE_F16) {
+                    lb_set_error("lb_program_create: op %lld: the tiny VAE input stage is fp16-only", (long long)i);
+                    e = 2;
+                }
+                break;
+            }
             default:
                 lb_set_error("lb_program_create: op %lld has unknown kind %d", (long long)i, ops[i].kind);
                 e = 2;
@@ -207,6 +219,12 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             case LB_OP_CONV_IN: {
                 const auto& a = o.u.conv;
                 e = lb_conv_in_dt(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, stream, o.dtype);
+                break;
+            }
+            case LB_OP_CONV_IN_ACT: {
+                const auto& a = o.u.conv_act;
+                e = lb_conv_in_act(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.act,
+                                   a.in_scale, stream, o.dtype);
                 break;
             }
             case LB_OP_CONV_OUT: {

@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .taesd import TinyVAEDecoderB200
 from .vae import VAEDecoderB200
 from .unet import UNetB200
 
@@ -66,13 +67,19 @@ class DiffusersHolder:
     def set_vae_dtype(self, vae_dtype):
         """Rebuild the VAE decoder with "fp16" or "bf16" storage (fp32 accumulation either way).  bf16 decodes VAEs
         whose activations overflow fp16, such as the stock SDXL VAE; a diffusers pipeline picks it from the VAE
-        config's force_upcast."""
+        config's force_upcast.  The tiny autoencoder (``pipe.vae_kind == "tiny"``, AutoencoderTiny) is fp16 only."""
         from .pipe import VAE_DTYPES
         if vae_dtype not in VAE_DTYPES:
             raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
         p = self.pipe
-        self.vae = VAEDecoderB200(p.vae_state_dict, p.vae_channels, p.vae_scaling_factor, self.device,
-                                  dtype=VAE_DTYPES[vae_dtype])
+        if getattr(p, "vae_kind", "kl") == "tiny":
+            if vae_dtype != "fp16":
+                raise ValueError(f"the tiny VAE decoder (AutoencoderTiny) runs in fp16 only (got {vae_dtype!r}): its "
+                                 "activations stay within fp16's range, and there is no bf16 build of it")
+            self.vae = TinyVAEDecoderB200(p.vae_state_dict, p.vae_config, p.vae_scaling_factor, self.device)
+        else:
+            self.vae = VAEDecoderB200(p.vae_state_dict, p.vae_channels, p.vae_scaling_factor, self.device,
+                                      dtype=VAE_DTYPES[vae_dtype])
         self.vae_dtype = vae_dtype
 
     def set_num_inference_steps(self, num_inference_steps):

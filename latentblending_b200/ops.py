@@ -144,13 +144,16 @@ _TILING = {"auto": 0, "box": _cabi.GEMM_TILE_BOX, "runs": _cabi.GEMM_TILE_RUNS}
 
 
 def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None, out=None,
-         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto", out_dtype=None):
+         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto", out_dtype=None,
+         depth_to_space=False):
     """Tensor-core GEMM / implicit-GEMM conv (lb_gemm).  a0: NHWC activation viewed as
     [B*H*W, >=a0_c] (row stride = a0.stride(0)); w: [N, K] packed weights.
     ``tiling``: "auto" (the M tiling with fewer tiles), "box" (pixel boxes) or "runs" (pixel runs); all give the
     same results.
     Element types come from the tensors: fp16 throughout, or bf16 a0 / w / a1 / bias / bias2 / res (LB_GEMM_BF16)
-    with a bf16 output, or an fp16 one when ``out_dtype`` (default: ``out``'s dtype, else a0's) is torch.float16."""
+    with a bf16 output, or an fp16 one when ``out_dtype`` (default: ``out``'s dtype, else a0's) is torch.float16.
+    ``depth_to_space`` (LB_GEMM_D2S2): nearest-2x upsample + 3x3 conv of the H x W map a0, with ``w`` the [4*Co, 9*C]
+    phase weights (``taesd.pack_d2s_weights``); the output is the [B*2H*2W, Co] NHWC map."""
     if tiling not in _TILING:
         raise ValueError(f"tiling must be one of {sorted(_TILING)} (got {tiling!r})")
     dev = _dev(a0)
@@ -162,8 +165,11 @@ def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bi
     elif out is not None and out.dtype != out_dtype:
         raise _cabi.LB200Error(f"gemm: out is {out.dtype}, out_dtype {out_dtype}")
     dmode = gemm_dtype_mode(a0, w, out_dtype, a1, bias, bias2, res)
+    if depth_to_space:
+        dmode |= _cabi.GEMM_D2S2
     if out is None:
-        out = torch.empty((M, n_out), dtype=out_dtype, device=a0.device)
+        shape = (4 * M, N // 4) if depth_to_space else (M, n_out)
+        out = torch.empty(shape, dtype=out_dtype, device=a0.device)
     d = _cabi.GemmDesc()
     d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(-2), a0_c
     if a1 is not None:
@@ -291,14 +297,20 @@ def linear_small(x, w, bias=None, addend=None, act_in=0, act_out=0, out=None):
     return out
 
 
-def conv_in(x_nchw, w_packed, bias, Cout, out=None):
-    """fp16 or bf16 (x, weights, bias and out of one type)."""
+def conv_in(x_nchw, w_packed, bias, Cout, out=None, act=0, in_scale=1.0):
+    """fp16 or bf16 (x, weights, bias and out of one type).  ``act`` 1 (fp16): the tiny VAE decoder's input stage,
+    tanh(x * in_scale / 3) * 3 before the conv and ReLU after it (lb_conv_in_act)."""
     dev = _dev(x_nchw)
     dt = dtype16(x_nchw, "conv_in x")
     B, Cin, H, W = x_nchw.shape
     if out is None:
         out = torch.empty((B * H * W, Cout), dtype=x_nchw.dtype, device=x_nchw.device)
     _same_dtype(x_nchw.dtype, "conv_in x / w / bias / out", w_packed, bias, out)
+    if act:
+        check(_cabi.load().lb_conv_in_act(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout,
+                                          ptr(out), out.stride(0), int(act), float(in_scale), stream_ptr(), dt),
+              "lb_conv_in_act")
+        return out
     check(_cabi.load().lb_conv_in_dt(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout, ptr(out),
                                      out.stride(0), stream_ptr(), dt), "lb_conv_in")
     return out

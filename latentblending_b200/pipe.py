@@ -159,6 +159,58 @@ def vae_param_shapes(channels=VAE_CHANNELS, latent=4):
     return P
 
 
+def tiny_vae_param_shapes(config=None):
+    """diffusers state_dict names (``decoder.`` stripped) -> shapes of an AutoencoderTiny decoder."""
+    from .taesd import decoder_layout, tiny_config
+    cfg = tiny_config(config)
+    ch = cfg["decoder_block_out_channels"]
+    P = OrderedDict()
+    for kind, idx, grp in decoder_layout(cfg):
+        c = ch[grp]
+        if kind == "block":
+            for j in (0, 2, 4):
+                P[f"layers.{idx}.conv.{j}.weight"] = (c, c, 3, 3)
+                P[f"layers.{idx}.conv.{j}.bias"] = (c,)
+        elif kind == "conv_in":
+            P[f"layers.{idx}.weight"] = (c, cfg["latent_channels"], 3, 3)
+            P[f"layers.{idx}.bias"] = (c,)
+        elif kind == "up_conv":
+            P[f"layers.{idx}.weight"] = (c, c, 3, 3)
+        else:
+            P[f"layers.{idx}.weight"] = (cfg["out_channels"], c, 3, 3)
+            P[f"layers.{idx}.bias"] = (cfg["out_channels"],)
+    return P
+
+
+def random_tiny_vae_state_dict(seed, device, config=None, dtype=torch.float16):
+    """Seeded tiny-VAE decoder weights whose frames are not degenerate.  35 convolutions and 31 ReLUs collapse a
+    uniform(+-1/sqrt(fan_in)) init to a constant, so: every conv is He-uniform (+-sqrt(6/fan_in), variance 2/fan_in,
+    which keeps the second moment through a ReLU); the third conv of each block is damped by 0.3 so the residual
+    stream grows slowly; biases are 0.02 * uniform(+-1); the last conv is uniform(+-0.25/sqrt(fan_in)) with bias
+    0.5, i.e. a mid-grey frame with a spread of a few tens of uint8 levels (decode returns layers(x) * 2 - 1)."""
+    from .taesd import decoder_layout
+    g = torch.Generator(device=device).manual_seed(seed)
+    shapes = tiny_vae_param_shapes(config)
+    last = [idx for kind, idx, _ in decoder_layout(config) if kind == "conv_out"][0]
+    sd = OrderedDict()
+    for name, shape in shapes.items():
+        u = torch.rand(shape, generator=g, device=device) * 2 - 1
+        if len(shape) >= 2:
+            fan_in = shape[1] * shape[2] * shape[3]
+            if name == f"layers.{last}.weight":
+                t = u * (0.25 / math.sqrt(fan_in))
+            else:
+                t = u * math.sqrt(6.0 / fan_in)
+                if name.endswith(".conv.4.weight"):
+                    t = t * 0.3
+        elif name == f"layers.{last}.bias":
+            t = 0.5 + 0.02 * u
+        else:
+            t = 0.02 * u
+        sd[name] = t.to(dtype)
+    return sd
+
+
 _DAMPED = ("conv2.weight", "conv2.bias", "to_out.0.weight", "to_out.0.bias", "ff.net.2.weight", "ff.net.2.bias",
            "proj_out.weight", "proj_out.bias")
 
@@ -194,10 +246,17 @@ class SyntheticSDXLPipe:
 
     def __init__(self, name="stabilityai/stable-diffusion-xl-base-1.0", device="cuda:0", unet_cfg: UNetConfig = None,
                  seed=0, unet_state_dict=None, vae_state_dict=None, vae_channels=VAE_CHANNELS,
-                 lpips_state_dict=None, vae_dtype="fp16"):
-        """``vae_dtype``: "fp16" or "bf16", the storage type of the VAE decoder DiffusersHolder builds."""
+                 lpips_state_dict=None, vae_dtype="fp16", vae="kl"):
+        """``vae_dtype``: "fp16" or "bf16", the storage type of the VAE decoder DiffusersHolder builds.
+        ``vae``: "kl" (the SDXL AutoencoderKL decoder) or "tiny" (the AutoencoderTiny / TAESDXL decoder with its
+        default config, scaling_factor 1.0, fp16 only; ``vae_state_dict`` then holds its ``decoder.``-stripped
+        weights, seeded by ``random_tiny_vae_state_dict`` when omitted)."""
         if vae_dtype not in VAE_DTYPES:
             raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
+        if vae not in ("kl", "tiny"):
+            raise ValueError(f"vae must be 'kl' or 'tiny' (got {vae!r})")
+        if vae == "tiny" and vae_dtype != "fp16":
+            raise ValueError("the tiny VAE decoder runs in fp16 only (vae_dtype='fp16')")
         self._name_or_path = name
         self.device = torch.device(device)
         self._execution_device = self.device
@@ -207,10 +266,19 @@ class SyntheticSDXLPipe:
         self.scheduler = EulerTables("euler_ancestral" if turbo else "euler")
         self.unet_state_dict = unet_state_dict if unet_state_dict is not None else \
             random_state_dict(unet_param_shapes(self.unet_cfg), seed, self.device)
-        self.vae_channels = tuple(vae_channels)
-        self.vae_state_dict = vae_state_dict if vae_state_dict is not None else \
-            random_state_dict(vae_param_shapes(vae_channels), seed + 1, self.device, damp=0.3)
-        self.vae_scaling_factor = 0.13025
+        self.vae_kind = vae
+        if vae == "tiny":
+            from .taesd import DEFAULT_CONFIG
+            self.vae_config = dict(DEFAULT_CONFIG)
+            self.vae_channels = tuple(DEFAULT_CONFIG["decoder_block_out_channels"])
+            self.vae_state_dict = vae_state_dict if vae_state_dict is not None else \
+                random_tiny_vae_state_dict(seed + 1, self.device)
+            self.vae_scaling_factor = float(DEFAULT_CONFIG["scaling_factor"])
+        else:
+            self.vae_channels = tuple(vae_channels)
+            self.vae_state_dict = vae_state_dict if vae_state_dict is not None else \
+                random_state_dict(vae_param_shapes(vae_channels), seed + 1, self.device, damp=0.3)
+            self.vae_scaling_factor = 0.13025
         self.vae_dtype = vae_dtype
         self.lpips_state_dict = lpips_state_dict
         self.h2d_bytes = 0        # bytes of conditioning copied host->device (bench e2e)
@@ -250,6 +318,9 @@ class DiffusersSDXLPipe:
     ``_execution_device`` / ``_name_or_path`` / ``default_sample_size`` / ``vae_scale_factor``.
     ``vae_dtype`` follows the VAE config: "bf16" when it sets ``force_upcast`` (the stock SDXL VAE, where the reference
     decodes in fp32), "fp16" for an fp16-safe VAE that turns it off.
+    A ``pipe.vae`` of class ``AutoencoderTiny`` (``AutoencoderTiny.from_pretrained('madebyollin/taesdxl')``, as the
+    reference's examples swap in) selects the tiny decoder: ``vae_kind`` "tiny", its ``decoder.`` weights and config,
+    fp16.
     ``lpips_state_dict`` must be supplied (see INTEGRATION.md "LPIPS weights"): with real weights a random LPIPS
     network would silently steer the branch placement."""
     is_synthetic = False
@@ -290,12 +361,26 @@ class DiffusersSDXLPipe:
         self.scheduler = tables_from_diffusers_scheduler(pipe.scheduler)
         self.unet_state_dict = pipe.unet.state_dict()
         vsd = pipe.vae.state_dict()
-        self.vae_state_dict = OrderedDict((k[len("decoder."):] if k.startswith("decoder.") else k, v)
-                                          for k, v in vsd.items() if k.startswith(("decoder.", "post_quant_conv.")))
         vcfg = pipe.vae.config
-        self.vae_channels = tuple(vcfg["block_out_channels"] if "block_out_channels" in vcfg else vcfg.block_out_channels)
-        self.vae_scaling_factor = float(vcfg["scaling_factor"] if "scaling_factor" in vcfg else vcfg.scaling_factor)
-        self.vae_dtype = vae_dtype_from_config(vcfg)
+        if type(pipe.vae).__name__ == "AutoencoderTiny":
+            # the tiny autoencoder (e.g. madebyollin/taesdxl): its decoder only; fp16, the one precision it has here
+            from .taesd import check_config, check_state_dict
+            self.vae_kind = "tiny"
+            self.vae_config = check_config(vcfg)
+            self.vae_state_dict = OrderedDict((k[len("decoder."):], v) for k, v in vsd.items()
+                                              if k.startswith("decoder."))
+            check_state_dict(self.vae_state_dict, self.vae_config)
+            self.vae_channels = tuple(self.vae_config["decoder_block_out_channels"])
+            self.vae_scaling_factor = float(self.vae_config["scaling_factor"])
+            self.vae_dtype = "fp16"
+        else:
+            self.vae_kind = "kl"
+            self.vae_state_dict = OrderedDict((k[len("decoder."):] if k.startswith("decoder.") else k, v)
+                                              for k, v in vsd.items() if k.startswith(("decoder.", "post_quant_conv.")))
+            self.vae_channels = tuple(vcfg["block_out_channels"] if "block_out_channels" in vcfg
+                                      else vcfg.block_out_channels)
+            self.vae_scaling_factor = float(vcfg["scaling_factor"] if "scaling_factor" in vcfg else vcfg.scaling_factor)
+            self.vae_dtype = vae_dtype_from_config(vcfg)
         self.lpips_state_dict = lpips_state_dict if lpips_state_dict is not None else getattr(pipe, "lpips_state_dict", None)
         self.h2d_bytes = 0
 

@@ -81,10 +81,12 @@ class Program:
 
     # -- op emitters (mirror latentblending_b200.ops, but record instead of launching) --------
     def gemm(self, a0, w, N, B, H, W, out, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None,
-             mode=0, static_w=True, relu=False, ln=None, stats_out=None):
+             mode=0, static_w=True, relu=False, ln=None, stats_out=None, depth_to_space=False):
         """``static_w``: ``w`` holds model weights (not written by the preceding op), so the kernel may fetch its
         first tiles before the preceding kernel has finished (LB_GEMM_STATIC_W).  Pass False when an activation
         is used as the B operand.
+        ``depth_to_space``: nearest-2x upsample + 3x3 conv as one GEMM (LB_GEMM_D2S2): ``w`` holds the four phase
+        filters [4*Co, 9*C], ``out`` the [B*2H*2W, Co] upsampled map.
         ``ln``: dict(stats=[M,parts,2] fp32, csum=[N] fp32, bias=[N] fp32, eps) -- LayerNorm folded into this GEMM
         (``w`` must already hold w*gamma; see include/lb200.h).  ``stats_out``: [M,parts,2] fp32 buffer that receives
         this GEMM's per-row partial sums for a following LN-folded GEMM (parts = self.gemm_stats_parts(...)).
@@ -104,6 +106,8 @@ class Program:
             d.res, d.res_ld = _p(res), res.stride(0)
         d.out, d.out_ld = _p(out), out.stride(0)
         d.mode = mode | (GEMM_STATIC_W if static_w else 0) | (GEMM_RELU if relu else 0) | dmode
+        if depth_to_space:
+            d.mode |= _cabi.GEMM_D2S2
         if ln is not None:
             st = ln["stats"]
             assert st.dtype == torch.float32 and st.dim() == 3 and st.shape[2] == 2 and st.is_contiguous()
@@ -193,6 +197,14 @@ class Program:
         B, Cin, H, W = x_nchw.shape
         d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
         d.out, d.ld_out = _p(out), out.stride(0)
+        self.hold(x_nchw, w, bias, out)
+
+    def conv_in_act(self, x_nchw, w, bias, Cout, out, act, in_scale=1.0, dtype=0):
+        """lb_conv_in_act: ``act`` 1 is the tiny VAE decoder's input stage (tanh clamp, conv, ReLU)."""
+        d = self._new_dt(_cabi.OP_CONV_IN_ACT, dtype).u.conv_act
+        B, Cin, H, W = x_nchw.shape
+        d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
+        d.out, d.ld_out, d.act, d.in_scale = _p(out), out.stride(0), act, in_scale
         self.hold(x_nchw, w, bias, out)
 
     def conv_out(self, x, B, H, W, Cin, w, bias, Cout, out_nchw):

@@ -24,14 +24,57 @@ from .unet import Program, pack_conv_out8
 _DTYPES = {torch.float16: _cabi.DTYPE_F16, torch.bfloat16: _cabi.DTYPE_BF16}
 
 
-class VAEDecoderB200:
+class DecoderBase:
+    """What every native VAE decoder shares (this one and taesd.TinyVAEDecoderB200): one lowered program per latent
+    size (``_lower(h, w)``: an object with ``z_in``, ``prog`` and ``frame``), and the count of non-finite pixels the
+    post-process kernel saw (``_overflow_message(n)`` says what it means for the decoder)."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self.dev_index = self.device.index or 0
+        self._plans = {}
+        self.nonfinite = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.decodes_since_check = 0
+
+    def plan(self, h, w):
+        if (h, w) not in self._plans:
+            self._plans[(h, w)] = self._lower(h, w)
+        return self._plans[(h, w)]
+
+    @torch.no_grad()
+    def decode_to_u8(self, latents):
+        """latents [1,4,h,w] fp16 (CUDA) -> uint8 [8h,8w,3] frame on the device."""
+        assert latents.is_cuda and latents.shape[0] == 1, "VAE decode: one CUDA latent at a time"
+        _, _, h, w = latents.shape
+        pl = self.plan(h, w)
+        pl.z_in.copy_(latents)
+        pl.prog.run()
+        self.decodes_since_check += 1
+        return pl.frame.clone()
+
+    def overflow_count(self):
+        """Non-finite pixels seen by the post-process kernel since the last call (device->host read: call it at a
+        point that synchronises anyway).  The fp16 decoder stores fp16 where the reference upcasts the stock SDXL VAE to
+        fp32 (diffusers_holder.py:128-133); with weights that overflow fp16 this is > 0 and the frames are invalid."""
+        n = int(self.nonfinite.item())
+        if n:
+            self.nonfinite.zero_()
+        self.decodes_since_check = 0
+        return n
+
+    def check_overflow(self):
+        n = self.overflow_count()
+        if n:
+            raise _cabi.LB200Error(self._overflow_message(n))
+
+
+class VAEDecoderB200(DecoderBase):
     def __init__(self, state_dict, channels, scaling_factor, device, groups=32, dtype=torch.float16):
         """``dtype``: torch.float16 or torch.bfloat16, the storage type of weights and activations (fp32 accumulation
         either way).  Weights are cast once from the state dict's own dtype; folded biases are formed in fp32."""
         if dtype not in _DTYPES:
             raise ValueError(f"VAE decoder dtype must be torch.float16 or torch.bfloat16 (got {dtype})")
-        self.device = torch.device(device)
-        self.dev_index = self.device.index or 0
+        super().__init__(device)
         self.channels = tuple(channels)
         self.scaling_factor = scaling_factor
         self.groups = groups
@@ -92,47 +135,16 @@ class VAEDecoderB200:
         if dtype == torch.bfloat16 and W["conv_out.w8"] is None:
             raise _cabi.LB200Error("the bf16 VAE decoder runs conv_out as an N = 8 GEMM, which needs a multiple of 64 "
                                    f"channels there (got {W['conv_out.w'].shape[-1]})")
-        self._plans = {}
-        self.nonfinite = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.decodes_since_check = 0
+    def _lower(self, h, w):
+        return _VAELowering(self, h, w)
 
-    def plan(self, h, w):
-        if (h, w) not in self._plans:
-            self._plans[(h, w)] = _VAELowering(self, h, w)
-        return self._plans[(h, w)]
-
-    @torch.no_grad()
-    def decode_to_u8(self, latents):
-        """latents [1,4,h,w] fp16 (CUDA) -> uint8 [8h,8w,3] frame on the device."""
-        assert latents.is_cuda and latents.shape[0] == 1, "VAE decode: one CUDA latent at a time"
-        _, _, h, w = latents.shape
-        pl = self.plan(h, w)
-        pl.z_in.copy_(latents)
-        pl.prog.run()
-        self.decodes_since_check += 1
-        return pl.frame.clone()
-
-    def overflow_count(self):
-        """Non-finite pixels seen by the post-process kernel since the last call (device->host read: call it at a
-        point that synchronises anyway).  The fp16 decoder stores fp16 where the reference upcasts the stock SDXL VAE to
-        fp32 (diffusers_holder.py:128-133); with weights that overflow fp16 this is > 0 and the frames are invalid."""
-        n = int(self.nonfinite.item())
-        if n:
-            self.nonfinite.zero_()
-        self.decodes_since_check = 0
-        return n
-
-    def check_overflow(self):
-        n = self.overflow_count()
-        if n:
-            if self.dtype == torch.float16:
-                raise _cabi.LB200Error(
-                    f"VAE decode produced {n} non-finite pixels: these VAE weights overflow fp16 (the reference upcasts "
+    def _overflow_message(self, n):
+        if self.dtype == torch.float16:
+            return (f"VAE decode produced {n} non-finite pixels: these VAE weights overflow fp16 (the reference upcasts "
                     "the stock SDXL VAE to fp32, diffusers_holder.py:128-133); decode in bf16 instead "
                     "(DiffusersHolder.set_vae_dtype(\"bf16\"), chosen automatically when the VAE config sets "
                     "force_upcast) or use the fp16-safe SDXL VAE weights (madebyollin/sdxl-vae-fp16-fix)")
-            raise _cabi.LB200Error(f"VAE decode produced {n} non-finite pixels in bf16: the latents or the VAE weights "
-                                   "are not finite")
+        return f"VAE decode produced {n} non-finite pixels in bf16: the latents or the VAE weights are not finite"
 
 
 class _VAELowering:
