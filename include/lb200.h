@@ -19,13 +19,18 @@
  *    ([batch*height*width, channels] row-major); latents are NCHW like the
  *    reference's ``[1,4,h,w]`` tensors.
  *  - bf16 means bfloat16 (``__nv_bfloat16``: fp32's 8-bit exponent, 8-bit
- *    significand).  The VAE-decoder ops also exist in bf16 (LB_GEMM_BF16 and
- *    the ``*_dt`` entry points with dtype LB_DTYPE_BF16): the stock SDXL VAE's
- *    activations exceed fp16's range (the reference decodes it in fp32 when
- *    its config sets force_upcast, diffusers_holder.py:128-139), bf16's range
- *    is fp32's, and bf16 wgmma runs at the fp16 rate.  Every bf16 variant keeps
- *    the fp16 variant's layouts, strides, alignment rules and fp32 arithmetic;
- *    only the stored element type differs.
+ *    significand).  The VAE-decoder ops also exist in bf16: the stock SDXL
+ *    VAE's activations exceed fp16's range (the reference decodes it in fp32
+ *    when its config sets force_upcast, diffusers_holder.py:128-139), bf16's
+ *    range is fp32's, and bf16 wgmma runs at the fp16 rate.  lb_gemm takes its
+ *    types from its mode flags (LB_GEMM_BF16); every other op with a bf16
+ *    variant takes a trailing ``int dtype`` (LB_DTYPE_F16 or LB_DTYPE_BF16, the
+ *    element type of its 16-bit tensors; any other value is an error):
+ *    lb_groupnorm, lb_conv_in, lb_upsample_nearest, lb_latent_prep,
+ *    lb_softmax_rows, lb_postprocess_u8 and lb_nhwc_to_nchw.  A bf16 call keeps
+ *    the fp16 call's layouts, strides, alignment rules and fp32 arithmetic;
+ *    only the stored element type differs, except where an entry point says
+ *    otherwise.
  */
 #ifndef LB200_H
 #define LB200_H
@@ -37,9 +42,9 @@
 extern "C" {
 #endif
 
-#define LB_ABI_VERSION 2
+#define LB_ABI_VERSION 3
 
-/* element type of the ops that exist in both 16-bit formats (lb_op.dtype, the ``*_dt`` entry points) */
+/* element type of the ops that exist in both 16-bit formats (lb_op.dtype, the trailing ``dtype`` arguments) */
 enum { LB_DTYPE_F16 = 0, LB_DTYPE_BF16 = 1 };
 
 typedef struct lb_ctx lb_ctx;
@@ -160,7 +165,7 @@ typedef struct lb_gemm_desc {
  * a checkpoint whose activations overflow fp16 runs on it. */
 #define LB_GEMM_BF16 0x1000
 /* mode flag, only with LB_GEMM_BF16: bf16 operands, fp16 output (the VAE attention scores, whose fp16 rounding is 8x
- * finer than bf16's and whose magnitudes stay far inside fp16's range; lb_softmax_rows_dt reads them as fp16) */
+ * finer than bf16's and whose magnitudes stay far inside fp16's range; lb_softmax_rows reads them as fp16) */
 #define LB_GEMM_OUT_F16 0x2000
 /* mode flag: nearest-2x upsample followed by a 3x3 conv as ONE GEMM over the low-resolution map (the upsampling
  * convolutions of the tiny VAE decoder, AutoencoderTiny).  taps = 9 over a B x H x W map a0 with N = 4 * Co: the weight
@@ -202,17 +207,13 @@ int lb_attention(lb_ctx* ctx, const lb_attn_desc* desc, void* stream);
  * The GroupNorm workspace (lb_groupnorm_workspace_bytes) must be ZERO-FILLED once after allocation: it holds
  * per-batch "last block" counters which every call leaves at zero again; it may be shared by successive calls on
  * one stream.  Results do not depend on the batch size (row chunking is a function of HW only).
+ * lb_groupnorm in bf16: the same fp32 statistics and fixed-order reduction; the output is rounded to bf16 after the
+ * affine and again after SiLU.
  */
 size_t lb_groupnorm_workspace_bytes(lb_ctx* ctx, int B, int HW, int groups);
 int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
                  const void* gamma, const void* beta, float eps, int silu,
-                 void* out, int64_t ldo, void* workspace, void* stream);
-/* lb_groupnorm with x, gamma, beta and out of element type ``dtype`` (LB_DTYPE_BF16: bf16, the same fp32 statistics
- * and fixed-order reduction; the output is rounded to bf16 after the affine and again after SiLU).  lb_groupnorm is
- * its LB_DTYPE_F16 call. */
-int lb_groupnorm_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
-                    const void* gamma, const void* beta, float eps, int silu,
-                    void* out, int64_t ldo, void* workspace, void* stream, int dtype);
+                 void* out, int64_t ldo, void* workspace, void* stream, int dtype);
 int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
                  const void* gamma, const void* beta, float eps, void* out, int64_t ldo, void* stream);
 
@@ -224,20 +225,25 @@ int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
  *   (time_embedding, add_embedding, all resnet time_emb_proj in one launch);
  *   act: 0 none, 1 SiLU.
  * lb_conv_in / lb_conv_out: the 4->C0 and C0->4 3x3 convolutions at the NCHW
- *   latent boundary.  lb_upsample2x: nearest 2x (Upsample2D).  lb_im2col_s2: patch
- *   matrix of the stride-2 Downsample2D convs (then lb_gemm); its output is
- *   ceil(H/2) x ceil(W/2), so any H and W.
+ *   latent boundary.  lb_conv_in's ``act`` chooses an input transform and an
+ *   output activation:
+ *   act 0: none (in_scale unused); x, w_packed, bias and out of type ``dtype``;
+ *   act 1: the tiny VAE decoder's input stage (AutoencoderTiny:
+ *          decoder(latents / scaling_factor), whose first steps are
+ *          tanh(z / 3) * 3, Conv2d(4, C, 3, padding=1), ReLU).  Each input v
+ *          becomes h(h(tanh(h(h(v * in_scale) / 3))) * 3), h = rounding to
+ *          fp16 (the fp16 roundings of the reference's ``/ scaling_factor``,
+ *          ``/ 3``, ``tanh`` and ``* 3``; in_scale = 1 / scaling_factor), then
+ *          the 3x3 conv + bias, then max(., 0).  fp16 only.
  * lb_upsample_nearest: F.interpolate(size=(Ho, Wo), mode="nearest") of an H x W
  *   map for Ho in {2H-1, 2H} and Wo in {2W-1, 2W} (any other size is an error):
- *   the Upsample2D of an up block whose skip level has an odd side (diffusers'
+ *   Ho = 2H, Wo = 2W is the nearest 2x of Upsample2D; the cropped sizes are the
+ *   Upsample2D of an up block whose skip level has an odd side (diffusers'
  *   forward_upsample_size, latent sides not divisible by 2^(levels-1)).  Output
  *   pixel (yo, xo) is input pixel (yo >> 1, xo >> 1), i.e. nearest 2x cropped to
- *   Ho x Wo.  lb_upsample2x is the Ho = 2H, Wo = 2W case.  C and both row strides
- *   multiples of 8.
- * The ``*_dt`` variants take the element type as a trailing ``dtype``; the
- *   plain entry points are their LB_DTYPE_F16 calls.  lb_conv_in_dt with
- *   LB_DTYPE_BF16: x, w_packed, bias and out are bf16.  lb_upsample_nearest_dt
- *   copies 16-byte channel vectors, so it is the same kernel for both types.
+ *   Ho x Wo.  C and both row strides multiples of 8.
+ * lb_im2col_s2: patch matrix of the stride-2 Downsample2D convs (then lb_gemm);
+ *   its output is ceil(H/2) x ceil(W/2), so any H and W.
  */
 int lb_embed_inputs(lb_ctx* ctx, float t, const void* text_embeds, const void* time_ids, int B,
                     int dim_t, int pooled, int dim_a, void* temb_in, void* add_in, void* stream);
@@ -245,28 +251,11 @@ int lb_linear_small(lb_ctx* ctx, const void* x, int64_t ldx, int M, int K, const
                     const void* bias, const void* addend, int64_t ldadd, int act_in, int act_out,
                     void* out, int64_t ldo, int N, void* stream);
 int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-               const void* bias, int Cout, void* out, int64_t ldo, void* stream);
+               const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream, int dtype);
 int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,
                 const void* bias, int Cout, void* out_nchw, void* stream);
-int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
-                  void* stream);
 int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
-                        int Ho, int Wo, void* stream);
-int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                  const void* bias, int Cout, void* out, int64_t ldo, void* stream, int dtype);
-int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
-                           int64_t ldo, int Ho, int Wo, void* stream, int dtype);
-/* lb_conv_in_act: lb_conv_in_dt with an input transform and an output activation chosen by ``act``:
- *   act 0: lb_conv_in_dt itself (in_scale unused);
- *   act 1: the tiny VAE decoder's input stage (AutoencoderTiny: decoder(latents / scaling_factor), whose first
- *          steps are tanh(z / 3) * 3, Conv2d(4, C, 3, padding=1), ReLU).  Each input v becomes
- *          h(h(tanh(h(h(v * in_scale) / 3))) * 3), h = rounding to fp16 (the fp16 roundings of the reference's
- *          ``/ scaling_factor``, ``/ 3``, ``tanh`` and ``* 3``; in_scale = 1 / scaling_factor), then the 3x3 conv +
- *          bias, then max(., 0).  fp16 only (dtype LB_DTYPE_F16).
- * Same layouts and limits as lb_conv_in. */
-int lb_conv_in_act(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                   const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream,
-                   int dtype);
+                        int Ho, int Wo, void* stream, int dtype);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
 
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
@@ -278,33 +267,24 @@ int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, in
  *   (optional, device int) is incremented by the number of NaN/Inf pixels: the decoder runs in fp16 where the reference
  *   upcasts the stock SDXL VAE to fp32 because it "overflows in float16" (diffusers_holder.py:128-133); an overflow
  *   anywhere upstream reaches the image as Inf/NaN and is reported instead of silently producing a black frame.
- * The ``*_dt`` variants take the element type as a trailing ``dtype`` (the plain entry points are their LB_DTYPE_F16
- * calls).  With LB_DTYPE_BF16 (the bf16 decoder of a VAE that overflows fp16):
- *   lb_latent_prep_dt: fp16 latents in, bf16 out;
- *   lb_softmax_rows_dt: fp16 scores in (lb_gemm with LB_GEMM_BF16 | LB_GEMM_OUT_F16), bf16 probabilities out; in
+ * With LB_DTYPE_BF16 (the bf16 decoder of a VAE that overflows fp16):
+ *   lb_latent_prep: fp16 latents in, bf16 out;
+ *   lb_softmax_rows: fp16 scores in (lb_gemm with LB_GEMM_BF16 | LB_GEMM_OUT_F16), bf16 probabilities out; in
  *     place too (out == x, ldo == ld: every element is read before the same thread overwrites its 2 bytes);
- *   lb_postprocess_u8_dt: bf16 image in; non-finite pixels are still counted;
- *   lb_nhwc_to_nchw_dt: bf16 in and out.
+ *   lb_postprocess_u8: bf16 image in; non-finite pixels are still counted.
  */
 int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
-                   const void* bias_f32, void* out_nchw, void* stream);
+                   const void* bias_f32, void* out_nchw, void* stream, int dtype);
 int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
-                    void* stream);
+                    void* stream, int dtype);
 int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
-                      int* nonfinite_count_dev, void* stream);
-int lb_latent_prep_dt(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
-                      const void* bias_f32, void* out_nchw, void* stream, int dtype);
-int lb_softmax_rows_dt(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
-                       void* stream, int dtype);
-int lb_postprocess_u8_dt(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
-                         int* nonfinite_count_dev, void* stream, int dtype);
+                      int* nonfinite_count_dev, void* stream, int dtype);
 /* lb_nhwc_to_nchw: the first C (<= 8) columns of NHWC rows [B*hw, ld] -> NCHW [B, C, hw].  The C0 -> 4 (UNet eps) and
  * C0 -> 3 (VAE RGB) output convolutions run as lb_gemm with an 8-row zero-padded weight matrix (N = 8); this puts the
  * result back into the reference's [B,C,H,W] tensor layout.  (lb_conv_out is the direct kernel for widths that are not
  * multiples of 64.) */
-int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream);
-int lb_nhwc_to_nchw_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream,
-                       int dtype);
+int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream,
+                    int dtype);
 
 /* ---- LPIPS-AlexNet branch-placement metric (SURVEY section 8f next #2; blending_engine.py:744-758, lpips==0.1.4) ----
  * The five AlexNet convolutions run on lb_gemm (LB_GEMM_RELU) over patch matrices:
@@ -340,17 +320,14 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * lb_program_run replays it on ``stream`` (``t`` = the timestep fed to
  * LB_OP_EMBED_INPUTS).  Replaces the module walk of pipe.unet(...)
  * (diffusers_holder.py:336-344).
- * lb_op.dtype: the element type (LB_DTYPE_*) of GROUPNORM, LATENT_PREP, CONV_IN, CONV_IN_ACT, UPSAMPLE2X,
- * NHWC_TO_NCHW, POSTPROCESS_U8 and SOFTMAX_ROWS (for SOFTMAX_ROWS the output's: see lb_softmax_rows_dt), i.e. which
- * ``*_dt`` call the record makes.  It must be 0 for every other kind (a GEMM takes its types from its mode flags).
- * LB_OP_CONV_IN_ACT: lb_conv_in_act (record u.conv_act).
+ * lb_op.dtype: the ``dtype`` argument of the record's call for the kinds whose entry point takes one (above); it must
+ * be 0 for every other kind (a GEMM takes its types from its mode flags).  Kind 18 is retired.
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
-    LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_CONV_OUT = 8, LB_OP_UPSAMPLE2X = 9, LB_OP_IM2COL_S2 = 10,
+    LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_CONV_OUT = 8, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
-    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17,
-    LB_OP_CONV_IN_ACT = 18
+    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17
 };
 typedef struct lb_op {
     int32_t kind;
@@ -365,12 +342,10 @@ typedef struct lb_op {
                  void* temb_in; void* add_in; } embed;
         struct { const void* x; int64_t ldx; int32_t M, K; const void* w; int64_t ldw; const void* bias;
                  const void* addend; int64_t ldadd; int32_t act_in, act_out; void* out; int64_t ldo; int32_t N; } lin;
+        /* CONV_IN, CONV_OUT (act, in_scale: lb_conv_in's; unused by CONV_OUT) */
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
-                 int32_t Cout; void* out; int64_t ld_out; } conv;
-        /* CONV_IN_ACT: the CONV_IN fields, then lb_conv_in_act's act and in_scale */
-        struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
-                 int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale; } conv_act;
-        /* UPSAMPLE2X: output Ho x Wo (0 = 2H / 2W; see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
+                 int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale; } conv;
+        /* UPSAMPLE_NEAREST: output Ho x Wo (see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
         struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; int32_t Ho, Wo; } resample;
         /* LATENT_PREP: x,w,bias,out,B,C,n=h*w; SOFTMAX_ROWS: x,ld_x,out,ld_out,n=rows,C=cols;
          * POSTPROCESS_U8: x,out,B,C,n=h*w, w = optional device int counter of non-finite pixels;

@@ -65,16 +65,13 @@ class _LinOp(ctypes.Structure):
 
 class _ConvOp(ctypes.Structure):
     _fields_ = [("x", c_void_p), ("ld_x", c_int64), ("B", c_int32), ("Cin", c_int32), ("H", c_int32), ("W", c_int32),
-                ("w", c_void_p), ("bias", c_void_p), ("Cout", c_int32), ("out", c_void_p), ("ld_out", c_int64)]
-
-
-class _ConvActOp(ctypes.Structure):
-    _fields_ = _ConvOp._fields_ + [("act", c_int32), ("in_scale", c_float)]
+                ("w", c_void_p), ("bias", c_void_p), ("Cout", c_int32), ("out", c_void_p), ("ld_out", c_int64),
+                ("act", c_int32), ("in_scale", c_float)]
 
 
 class _ResampleOp(ctypes.Structure):
     _fields_ = [("x", c_void_p), ("ld_x", c_int64), ("B", c_int32), ("H", c_int32), ("W", c_int32), ("C", c_int32),
-                ("out", c_void_p), ("ld_out", c_int64), ("Ho", c_int32), ("Wo", c_int32)]   # 0 = 2H / 2W
+                ("out", c_void_p), ("ld_out", c_int64), ("Ho", c_int32), ("Wo", c_int32)]
 
 
 class _AuxOp(ctypes.Structure):
@@ -89,8 +86,7 @@ class _PatchOp(ctypes.Structure):
 
 class _OpUnion(ctypes.Union):
     _fields_ = [("gemm", GemmDesc), ("attn", AttnDesc), ("norm", _NormOp), ("embed", _EmbedOp), ("lin", _LinOp),
-                ("conv", _ConvOp), ("resample", _ResampleOp), ("aux", _AuxOp), ("patch", _PatchOp),
-                ("conv_act", _ConvActOp)]
+                ("conv", _ConvOp), ("resample", _ResampleOp), ("aux", _AuxOp), ("patch", _PatchOp)]
 
 
 class Op(ctypes.Structure):
@@ -105,11 +101,11 @@ GEMM_TILE_RUNS = 0x800    # LB_GEMM_TILE_RUNS: force the pixel-run M tiling
 GEMM_BF16 = 0x1000        # LB_GEMM_BF16: bf16 operands, bias, residual and output
 GEMM_OUT_F16 = 0x2000     # LB_GEMM_OUT_F16 (with GEMM_BF16): fp16 output
 GEMM_D2S2 = 0x4000        # LB_GEMM_D2S2: nearest-2x upsample + 3x3 conv as one GEMM, depth-to-space store
-DTYPE_F16, DTYPE_BF16 = 0, 1    # LB_DTYPE_F16 / LB_DTYPE_BF16: lb_op.dtype and the *_dt entry points
+DTYPE_F16, DTYPE_BF16 = 0, 1    # LB_DTYPE_F16 / LB_DTYPE_BF16: lb_op.dtype and the trailing dtype arguments
 (OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN, OP_CONV_OUT,
- OP_UPSAMPLE2X, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
- OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_CONV_IN_ACT) = range(1, 19)
-CONV_IN_PLAIN, CONV_IN_TINY_VAE = 0, 1     # lb_conv_in_act's act
+ OP_UPSAMPLE_NEAREST, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
+ OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = range(1, 18)
+CONV_IN_PLAIN, CONV_IN_TINY_VAE = 0, 1     # lb_conv_in's act
 
 
 # name -> (restype, argtypes); mirrors include/lb200.h one to one
@@ -139,9 +135,7 @@ SIGNATURES = {
     "lb_attention": (c_int, [c_void_p, ctypes.POINTER(AttnDesc), c_void_p]),
     "lb_groupnorm_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int]),
     "lb_groupnorm": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
-                             c_int, c_void_p, c_int64, c_void_p, c_void_p]),
-    "lb_groupnorm_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
-                                c_int, c_void_p, c_int64, c_void_p, c_void_p, c_int]),
+                             c_int, c_void_p, c_int64, c_void_p, c_void_p, c_int]),
     "lb_layernorm": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p, c_float, c_void_p,
                              c_int64, c_void_p]),
     "lb_embed_inputs": (c_int, [c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
@@ -149,28 +143,17 @@ SIGNATURES = {
     "lb_linear_small": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
                                 c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_void_p]),
     "lb_conv_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
-                           c_int64, c_void_p]),
-    "lb_conv_in_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
-                              c_int64, c_void_p, c_int]),
-    "lb_conv_in_act": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
-                               c_int64, c_int, c_float, c_void_p, c_int]),
+                           c_int64, c_int, c_float, c_void_p, c_int]),
     "lb_conv_out": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                             c_void_p, c_void_p]),
-    "lb_upsample2x": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
-                                    c_int, c_void_p]),
-    "lb_upsample_nearest_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64,
-                                       c_int, c_int, c_void_p, c_int]),
+                                    c_int, c_void_p, c_int]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "lb_latent_prep": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "lb_softmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p]),
-    "lb_postprocess_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
-    "lb_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_void_p, c_void_p]),
-    "lb_latent_prep_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
-                                  c_int]),
-    "lb_softmax_rows_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p, c_int]),
-    "lb_postprocess_u8_dt": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int]),
-    "lb_nhwc_to_nchw_dt": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_void_p, c_void_p, c_int]),
+    "lb_latent_prep": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                               c_int]),
+    "lb_softmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int64, c_void_p, c_int]),
+    "lb_postprocess_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int]),
+    "lb_nhwc_to_nchw": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_void_p, c_void_p, c_int]),
     "lb_lpips_im2col_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_float),
                                    ctypes.POINTER(c_float), c_void_p, c_int64, c_void_p]),
     "lb_im2col": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -208,7 +191,7 @@ def load():
             fn = getattr(lib, name)       # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args
-        if lib.lb_abi_version() != 2:
+        if lib.lb_abi_version() != 3:
             raise LB200Error("liblb200.so ABI version mismatch")
         _lib = lib
     return _lib

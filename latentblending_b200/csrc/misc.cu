@@ -110,7 +110,7 @@ linear_small_kernel(const __half* __restrict__ x, long long ldx, int M, int K, c
 
 // ---- conv_in: NCHW [B,Cin<=8,H,W] -> NHWC [B*H*W, Cout], 3x3 pad 1 -------------------------------
 // weights packed [ky][kx][cin][Cout] fp16 (bf16 in the bf16 variant) so a lane reads 8 consecutive output channels.
-// kTiny (lb_conv_in_act act 1, fp16): the tiny VAE decoder's input stage -- every input v is clamped to
+// kTiny (lb_conv_in act 1, fp16): the tiny VAE decoder's input stage -- every input v is clamped to
 // h(h(tanh(h(h(v * in_scale) / 3))) * 3) (h: fp16 rounding, at the reference's points), and ReLU follows the conv.
 __device__ __forceinline__ float tiny_vae_input(float v, float in_scale) {
     const float z = lb_round_h(v * in_scale);
@@ -343,63 +343,44 @@ extern "C" int lb_linear_small(lb_ctx* ctx, const void* x, int64_t ldx, int M, i
     return 0;
 }
 
-template <typename T>
+// One launcher for both conv_in kernels; ``extra`` is the kernel's arguments after ldo.
+template <typename T, auto kKernel, typename... Extra>
 static int conv_in_launch(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                          const void* bias, int Cout, void* out, int64_t ldo, void* stream) {
+                          const void* bias, int Cout, void* out, int64_t ldo, void* stream, Extra... extra) {
     LB_REQUIRE(ctx && x_nchw && w_packed && bias && out, "lb_conv_in: null argument");
     LB_REQUIRE(Cin >= 1 && Cin <= 8 && Cout % 8 == 0 && ldo % 8 == 0, "lb_conv_in: Cin<=8, Cout%%8==0 required");
     const int smem = 9 * Cin * Cout * 2;
     LB_REQUIRE(smem <= 96 * 1024, "lb_conv_in: weights do not fit shared memory");
-    static bool attr = false;
+    static bool attr = false;      // one flag per kernel (per instantiation)
     if (!attr) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_in_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        LB_CHECK_CUDA(cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         attr = true;
     }
     const long long npix = (long long)B * H * W;
     unsigned grid = (unsigned)lb_ceil_div(npix, kThreads / 32);
     if (grid > (unsigned)ctx->sm_count * 4) grid = ctx->sm_count * 4;
-    lb_launch_pdl(conv_in_kernel<T>, grid, kThreads, smem, lb_stream(stream), (const T*)x_nchw, B, Cin, H, W,
-                  (const T*)w_packed, (const T*)bias, Cout, (T*)out, ldo);
+    lb_launch_pdl(kKernel, grid, kThreads, smem, lb_stream(stream), (const T*)x_nchw, B, Cin, H, W,
+                  (const T*)w_packed, (const T*)bias, Cout, (T*)out, (long long)ldo, extra...);
     LB_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int lb_conv_in_dt(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                             const void* bias, int Cout, void* out, int64_t ldo, void* stream, int dtype) {
-    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_conv_in: unknown dtype %d", dtype);
-    return dtype == LB_DTYPE_BF16
-               ? conv_in_launch<__nv_bfloat16>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream)
-               : conv_in_launch<__half>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream);
 }
 
 extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                          const void* bias, int Cout, void* out, int64_t ldo, void* stream) {
-    return lb_conv_in_dt(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream, LB_DTYPE_F16);
-}
-
-extern "C" int lb_conv_in_act(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
-                              const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream,
-                              int dtype) {
-    LB_REQUIRE(act == 0 || act == 1, "lb_conv_in_act: unknown act %d (0 = plain, 1 = tiny VAE input stage)", act);
-    if (act == 0) return lb_conv_in_dt(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo, stream, dtype);
-    LB_REQUIRE(dtype == LB_DTYPE_F16, "lb_conv_in_act: the tiny VAE input stage (act 1) is fp16-only (dtype %d)", dtype);
-    LB_REQUIRE(ctx && x_nchw && w_packed && bias && out, "lb_conv_in_act: null argument");
-    LB_REQUIRE(Cin >= 1 && Cin <= 8 && Cout % 8 == 0 && ldo % 8 == 0, "lb_conv_in_act: Cin<=8, Cout%%8==0 required");
-    LB_REQUIRE(isfinite(in_scale), "lb_conv_in_act: in_scale must be finite");
-    const int smem = 9 * Cin * Cout * 2;
-    LB_REQUIRE(smem <= 96 * 1024, "lb_conv_in_act: weights do not fit shared memory");
-    static bool attr = false;
-    if (!attr) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_in_tiny_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr = true;
+                          const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream,
+                          int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_conv_in: unknown dtype %d", dtype);
+    LB_REQUIRE(act == 0 || act == 1, "lb_conv_in: unknown act %d (0 = plain, 1 = tiny VAE input stage)", act);
+    if (act == 1) {
+        LB_REQUIRE(dtype == LB_DTYPE_F16, "lb_conv_in: the tiny VAE input stage (act 1) is fp16-only (dtype %d)", dtype);
+        LB_REQUIRE(isfinite(in_scale), "lb_conv_in: in_scale must be finite");
+        return conv_in_launch<__half, conv_in_tiny_kernel>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo,
+                                                           stream, in_scale);
     }
-    const long long npix = (long long)B * H * W;
-    unsigned grid = (unsigned)lb_ceil_div(npix, kThreads / 32);
-    if (grid > (unsigned)ctx->sm_count * 4) grid = ctx->sm_count * 4;
-    lb_launch_pdl(conv_in_tiny_kernel, grid, kThreads, smem, lb_stream(stream), (const __half*)x_nchw, B, Cin, H, W,
-                  (const __half*)w_packed, (const __half*)bias, Cout, (__half*)out, (long long)ldo, in_scale);
-    LB_LAUNCH_CHECK();
-    return 0;
+    if (dtype == LB_DTYPE_BF16)
+        return conv_in_launch<__nv_bfloat16, conv_in_kernel<__nv_bfloat16>>(ctx, x_nchw, B, Cin, H, W, w_packed, bias,
+                                                                            Cout, out, ldo, stream);
+    return conv_in_launch<__half, conv_in_kernel<__half>>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo,
+                                                          stream);
 }
 
 extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,
@@ -424,8 +405,8 @@ extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Ci
 }
 
 // the kernel moves 16-byte channel vectors, so fp16 and bf16 maps share it
-extern "C" int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
-                                      int64_t ldo, int Ho, int Wo, void* stream, int dtype) {
+extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                                   int64_t ldo, int Ho, int Wo, void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_upsample_nearest: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x && out, "lb_upsample_nearest: null argument");
     LB_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0, "lb_upsample_nearest: C and strides must be multiples of 8");
@@ -437,16 +418,6 @@ extern "C" int lb_upsample_nearest_dt(lb_ctx* ctx, const void* x, int64_t ld, in
                   (const __half*)x, ld, B, H, W, C, (__half*)out, ldo, Ho, Wo);
     LB_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
-                                   int64_t ldo, int Ho, int Wo, void* stream) {
-    return lb_upsample_nearest_dt(ctx, x, ld, B, H, W, C, out, ldo, Ho, Wo, stream, LB_DTYPE_F16);
-}
-
-extern "C" int lb_upsample2x(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
-                             void* stream) {
-    return lb_upsample_nearest(ctx, x, ld, B, H, W, C, out, ldo, 2 * H, 2 * W, stream);
 }
 
 extern "C" int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream) {
@@ -599,8 +570,8 @@ postprocess_u8_kernel(const T* __restrict__ img, int B, int C, long long hw, uin
 }
 }  // namespace
 
-extern "C" int lb_latent_prep_dt(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
-                                 const void* bias_f32, void* out_nchw, void* stream, int dtype) {
+extern "C" int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
+                              const void* bias_f32, void* out_nchw, void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_latent_prep: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x_nchw && w_f32 && bias_f32 && out_nchw, "lb_latent_prep: null argument");
     LB_REQUIRE(C >= 1 && C <= 8, "lb_latent_prep: C must be <= 8");
@@ -615,13 +586,8 @@ extern "C" int lb_latent_prep_dt(lb_ctx* ctx, const void* x_nchw, int B, int C, 
     return 0;
 }
 
-extern "C" int lb_latent_prep(lb_ctx* ctx, const void* x_nchw, int B, int C, int64_t hw, const void* w_f32,
-                              const void* bias_f32, void* out_nchw, void* stream) {
-    return lb_latent_prep_dt(ctx, x_nchw, B, C, hw, w_f32, bias_f32, out_nchw, stream, LB_DTYPE_F16);
-}
-
-extern "C" int lb_softmax_rows_dt(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out,
-                                  int64_t ldo, void* stream, int dtype) {
+extern "C" int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out,
+                               int64_t ldo, void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_softmax_rows: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x && out, "lb_softmax_rows: null argument");
     LB_REQUIRE(cols >= 0 && ld % 8 == 0 && ldo % 8 == 0 && lb_aligned16(x) && lb_aligned16(out),
@@ -638,14 +604,9 @@ extern "C" int lb_softmax_rows_dt(lb_ctx* ctx, const void* x, int64_t ld, int64_
     return 0;
 }
 
-extern "C" int lb_softmax_rows(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int cols, void* out, int64_t ldo,
-                               void* stream) {
-    return lb_softmax_rows_dt(ctx, x, ld, rows, cols, out, ldo, stream, LB_DTYPE_F16);
-}
-
 // copies 2-byte elements: the same kernel for fp16 and bf16
-extern "C" int lb_nhwc_to_nchw_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
-                                  void* stream, int dtype) {
+extern "C" int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
+                               void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_nhwc_to_nchw: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && x && out_nchw, "lb_nhwc_to_nchw: null argument");
     LB_REQUIRE(C >= 1 && C <= 8 && ld % 8 == 0 && ld >= 8 && lb_aligned16(x), "lb_nhwc_to_nchw: C <= 8, row stride a "
@@ -656,13 +617,8 @@ extern "C" int lb_nhwc_to_nchw_dt(lb_ctx* ctx, const void* x, int64_t ld, int B,
     return 0;
 }
 
-extern "C" int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw,
-                               void* stream) {
-    return lb_nhwc_to_nchw_dt(ctx, x, ld, B, C, hw, out_nchw, stream, LB_DTYPE_F16);
-}
-
-extern "C" int lb_postprocess_u8_dt(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
-                                    int* nonfinite_count_dev, void* stream, int dtype) {
+extern "C" int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
+                                 int* nonfinite_count_dev, void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_postprocess_u8: unknown dtype %d", dtype);
     LB_REQUIRE(ctx && img_nchw && out_u8_nhwc, "lb_postprocess_u8: null argument");
     const unsigned grid = grid_for((long long)B * hw * C, ctx->sm_count);
@@ -674,9 +630,4 @@ extern "C" int lb_postprocess_u8_dt(lb_ctx* ctx, const void* img_nchw, int B, in
                       hw, (uint8_t*)out_u8_nhwc, nonfinite_count_dev);
     LB_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t hw, void* out_u8_nhwc,
-                                 int* nonfinite_count_dev, void* stream) {
-    return lb_postprocess_u8_dt(ctx, img_nchw, B, C, hw, out_u8_nhwc, nonfinite_count_dev, stream, LB_DTYPE_F16);
 }

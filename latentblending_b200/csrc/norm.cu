@@ -316,22 +316,15 @@ static int groupnorm_launch(lb_ctx* ctx, const void* x, int64_t ld, int B, int H
     return 0;
 }
 
-extern "C" int lb_groupnorm_dt(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
-                               const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
-                               void* workspace, void* stream, int dtype) {
+extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
+                            const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
+                            void* workspace, void* stream, int dtype) {
     LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_groupnorm: unknown dtype %d", dtype);
     return dtype == LB_DTYPE_BF16
                ? groupnorm_launch<__nv_bfloat16>(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo,
                                                  workspace, stream)
                : groupnorm_launch<__half>(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo, workspace,
                                           stream);
-}
-
-extern "C" int lb_groupnorm(lb_ctx* ctx, const void* x, int64_t ld, int B, int HW, int C, int groups,
-                            const void* gamma, const void* beta, float eps, int silu, void* out, int64_t ldo,
-                            void* workspace, void* stream) {
-    return lb_groupnorm_dt(ctx, x, ld, B, HW, C, groups, gamma, beta, eps, silu, out, ldo, workspace, stream,
-                           LB_DTYPE_F16);
 }
 
 extern "C" int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C, const void* gamma,

@@ -14,7 +14,7 @@
 
 // the op records are an ABI: a member may grow only inside the union's existing size (set by lb_gemm_desc)
 static_assert(sizeof(((lb_op*)nullptr)->u.resample) <= sizeof(lb_gemm_desc), "lb_op.u.resample outgrew the union");
-static_assert(sizeof(((lb_op*)nullptr)->u.conv_act) <= sizeof(lb_gemm_desc), "lb_op.u.conv_act outgrew the union");
+static_assert(sizeof(((lb_op*)nullptr)->u.conv) <= sizeof(lb_gemm_desc), "lb_op.u.conv outgrew the union");
 // lb_op.dtype took the place of a reserved int32: the record size and the union's offset are unchanged
 static_assert(sizeof(lb_op) == 8 + sizeof(lb_gemm_desc) && offsetof(lb_op, u) == 8, "lb_op layout changed");
 
@@ -30,8 +30,9 @@ int lb_set_scalar(float* dst_dev, float v, cudaStream_t st);
 // Replay mode.  The op list is static, so after one warm (direct) run the whole program is captured ONCE into a CUDA
 // graph -- every launch keeps its programmatic-dependent-launch edge -- and later runs are a single cudaGraphLaunch:
 // ~700-900 driver launches per UNet forward (2-4 ms of host time) become one, and the device's front end walks a
-// pre-built launch list.  The only run-time parameter, the timestep, lives in device memory (t_dev).  If capture is not
-// possible (another capture in flight, an unsupported driver) the program keeps launching directly.
+// pre-built launch list.  The only run-time parameter, the timestep, lives in device memory (t_dev, allocated when a
+// capture is first attempted: only the graph reads it).  If capture is not possible (another capture in flight, an
+// unsupported driver) the program keeps launching directly.
 struct lb_program {
     lb_ctx* ctx;
     struct Node {
@@ -46,6 +47,17 @@ struct lb_program {
     int runs = 0;
     int graph_state = 0;      // 0 not tried, 1 captured, -1 unavailable
 };
+
+// the kinds whose entry point takes a dtype argument (lb_op.dtype); every other kind needs dtype 0
+static bool kind_has_dtype(int kind) {
+    switch (kind) {
+        case LB_OP_GROUPNORM: case LB_OP_LATENT_PREP: case LB_OP_CONV_IN: case LB_OP_UPSAMPLE_NEAREST:
+        case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS:
+            return true;
+        default:
+            return false;
+    }
+}
 
 static bool lb_graphs_enabled() {
     static int v = -1;
@@ -63,20 +75,15 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
         nd.op = ops[i];
         nd.attn = nullptr;
         int e = 0;
-        switch (ops[i].kind) {     // the kinds that have a bf16 variant; every other kind needs dtype 0
-            case LB_OP_GROUPNORM: case LB_OP_LATENT_PREP: case LB_OP_CONV_IN: case LB_OP_UPSAMPLE2X:
-            case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS: case LB_OP_CONV_IN_ACT:
-                if (ops[i].dtype != LB_DTYPE_F16 && ops[i].dtype != LB_DTYPE_BF16) {
-                    lb_set_error("lb_program_create: op %lld has unknown dtype %d", (long long)i, ops[i].dtype);
-                    e = 2;
-                }
-                break;
-            default:
-                if (ops[i].dtype != LB_DTYPE_F16) {
-                    lb_set_error("lb_program_create: op %lld (kind %d) has no dtype %d variant (a GEMM takes its types "
-                                 "from its mode flags)", (long long)i, ops[i].kind, ops[i].dtype);
-                    e = 2;
-                }
+        if (kind_has_dtype(ops[i].kind)) {
+            if (ops[i].dtype != LB_DTYPE_F16 && ops[i].dtype != LB_DTYPE_BF16) {
+                lb_set_error("lb_program_create: op %lld has unknown dtype %d", (long long)i, ops[i].dtype);
+                e = 2;
+            }
+        } else if (ops[i].dtype != LB_DTYPE_F16) {
+            lb_set_error("lb_program_create: op %lld (kind %d) has no dtype %d variant (a GEMM takes its types "
+                         "from its mode flags)", (long long)i, ops[i].kind, ops[i].dtype);
+            e = 2;
         }
         if (!e) switch (ops[i].kind) {
             case LB_OP_GEMM:
@@ -85,13 +92,13 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_ATTENTION:
                 e = attn_plan_build_opaque(ctx, ops[i].u.attn, &nd.attn);
                 break;
-            case LB_OP_EMBED_INPUTS: case LB_OP_LINEAR_SMALL: case LB_OP_CONV_IN: case LB_OP_CONV_OUT:
-            case LB_OP_UPSAMPLE2X: case LB_OP_IM2COL_S2: case LB_OP_GROUPNORM: case LB_OP_LAYERNORM:
+            case LB_OP_EMBED_INPUTS: case LB_OP_LINEAR_SMALL: case LB_OP_CONV_OUT:
+            case LB_OP_UPSAMPLE_NEAREST: case LB_OP_IM2COL_S2: case LB_OP_GROUPNORM: case LB_OP_LAYERNORM:
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
                 break;
-            case LB_OP_CONV_IN_ACT: {
-                const auto& a = ops[i].u.conv_act;
+            case LB_OP_CONV_IN: {
+                const auto& a = ops[i].u.conv;
                 if (a.act != 0 && a.act != 1) {
                     lb_set_error("lb_program_create: op %lld: unknown conv_in act %d", (long long)i, a.act);
                     e = 2;
@@ -113,11 +120,6 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             delete prog;
             return e;
         }
-    }
-    if (cudaMalloc(&prog->t_dev, sizeof(float)) != cudaSuccess) {
-        cudaGetLastError();
-        prog->t_dev = nullptr;
-        prog->graph_state = -1;
     }
     *out = prog;
     return 0;
@@ -153,10 +155,11 @@ extern "C" int lb_program_run(lb_program* prog, float t, void* stream) {
             return program_launch_all(prog, t, nullptr, 0xFFFFFFFFu, stream);
         cudaGraph_t graph = nullptr;
         int e = 1;
+        if (prog->t_dev == nullptr && cudaMalloc(&prog->t_dev, sizeof(float)) != cudaSuccess) prog->t_dev = nullptr;
         if (prog->capture_stream == nullptr &&
             cudaStreamCreateWithFlags(&prog->capture_stream, cudaStreamNonBlocking) != cudaSuccess)
             prog->capture_stream = nullptr;
-        if (prog->capture_stream != nullptr &&
+        if (prog->t_dev != nullptr && prog->capture_stream != nullptr &&
             cudaStreamBeginCapture(prog->capture_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
             // nothing executes during capture: the launches only record the node list (with their PDL edges)
             e = program_launch_all(prog, t, prog->t_dev, 0xFFFFFFFFu, prog->capture_stream);
@@ -218,13 +221,8 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_CONV_IN: {
                 const auto& a = o.u.conv;
-                e = lb_conv_in_dt(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, stream, o.dtype);
-                break;
-            }
-            case LB_OP_CONV_IN_ACT: {
-                const auto& a = o.u.conv_act;
-                e = lb_conv_in_act(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.act,
-                                   a.in_scale, stream, o.dtype);
+                e = lb_conv_in(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.act, a.in_scale,
+                               stream, o.dtype);
                 break;
             }
             case LB_OP_CONV_OUT: {
@@ -232,10 +230,10 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
                 e = lb_conv_out(ctx, a.x, a.ld_x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, stream);
                 break;
             }
-            case LB_OP_UPSAMPLE2X: {
+            case LB_OP_UPSAMPLE_NEAREST: {
                 const auto& a = o.u.resample;
-                e = lb_upsample_nearest_dt(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out,
-                                           a.Ho ? a.Ho : 2 * a.H, a.Wo ? a.Wo : 2 * a.W, stream, o.dtype);
+                e = lb_upsample_nearest(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out, a.Ho, a.Wo, stream,
+                                        o.dtype);
                 break;
             }
             case LB_OP_IM2COL_S2: {
@@ -245,8 +243,8 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_GROUPNORM: {
                 const auto& a = o.u.norm;
-                e = lb_groupnorm_dt(ctx, a.x, a.ld_x, a.B, (int)a.rows, a.C, a.groups, a.gamma, a.beta, a.eps, a.silu,
-                                    a.out, a.ld_out, a.workspace, stream, o.dtype);
+                e = lb_groupnorm(ctx, a.x, a.ld_x, a.B, (int)a.rows, a.C, a.groups, a.gamma, a.beta, a.eps, a.silu,
+                                 a.out, a.ld_out, a.workspace, stream, o.dtype);
                 break;
             }
             case LB_OP_LAYERNORM: {
@@ -256,22 +254,22 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             }
             case LB_OP_LATENT_PREP: {
                 const auto& a = o.u.aux;
-                e = lb_latent_prep_dt(ctx, a.x, a.B, a.C, a.n, a.w, a.bias, a.out, stream, o.dtype);
+                e = lb_latent_prep(ctx, a.x, a.B, a.C, a.n, a.w, a.bias, a.out, stream, o.dtype);
                 break;
             }
             case LB_OP_SOFTMAX_ROWS: {
                 const auto& a = o.u.aux;
-                e = lb_softmax_rows_dt(ctx, a.x, a.ld_x, a.n, a.C, a.out, a.ld_out, stream, o.dtype);
+                e = lb_softmax_rows(ctx, a.x, a.ld_x, a.n, a.C, a.out, a.ld_out, stream, o.dtype);
                 break;
             }
             case LB_OP_POSTPROCESS_U8: {
                 const auto& a = o.u.aux;
-                e = lb_postprocess_u8_dt(ctx, a.x, a.B, a.C, a.n, a.out, (int*)const_cast<void*>(a.w), stream, o.dtype);
+                e = lb_postprocess_u8(ctx, a.x, a.B, a.C, a.n, a.out, (int*)const_cast<void*>(a.w), stream, o.dtype);
                 break;
             }
             case LB_OP_NHWC_TO_NCHW: {
                 const auto& a = o.u.aux;
-                e = lb_nhwc_to_nchw_dt(ctx, a.x, a.ld_x, a.B, a.C, a.n, a.out, stream, o.dtype);
+                e = lb_nhwc_to_nchw(ctx, a.x, a.ld_x, a.B, a.C, a.n, a.out, stream, o.dtype);
                 break;
             }
             case LB_OP_LPIPS_IM2COL_U8: {

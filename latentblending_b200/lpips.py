@@ -19,7 +19,7 @@ import torch
 
 from . import _cabi, ops
 from ._cabi import ctx
-from .unet import Program
+from .program import Program
 
 _LP_SHIFT = (-0.030, -0.088, -0.188)
 _LP_SCALE = (0.458, 0.448, 0.450)

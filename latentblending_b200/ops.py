@@ -1,15 +1,15 @@
 """Tensor-level wrappers over the C ABI (device memory and streams come from
 PyTorch; all arithmetic happens in liblb200.so).  Every function requires CUDA
-tensors and raises otherwise -- there is no CPU path."""
+tensors and raises otherwise -- there is no CPU path.  The wrappers of executor op kinds record one op into a fresh
+``Program`` and run it, so they go through the same records and create-time validation as the lowered programs."""
 import numpy as np
 import torch
 
 from . import _cabi
 from ._cabi import check, ctx, ptr, stream_ptr
+from .program import LAUNCHES, Program
 
 _DT = {torch.float16: 0, torch.float32: 1}
-_DT16 = {torch.float16: _cabi.DTYPE_F16, torch.bfloat16: _cabi.DTYPE_BF16}   # the ops with fp16 and bf16 variants
-LAUNCHES = [0]      # kernels of liblb200 launched through this module / Program.run (bench.py reports it)
 
 
 def _dev(t):
@@ -110,100 +110,39 @@ def cfg_euler_step(latents, eps, guidance, sigma, dt, sigma_up=0.0, noise=None, 
     return out
 
 
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-def dtype16(t, what="tensor"):
-    """LB_DTYPE_* of an fp16 / bf16 tensor; anything else raises."""
-    if t.dtype not in _DT16:
-        raise _cabi.LB200Error(f"{what} must be float16 or bfloat16 (got {t.dtype})")
-    return _DT16[t.dtype]
-
-
-def _same_dtype(dtype, what, *ts):
-    for t in ts:
-        if t is not None and t.dtype != dtype:
-            raise _cabi.LB200Error(f"{what}: mixed element types ({t.dtype} with {dtype})")
-
-
-def gemm_dtype_mode(a0, w, out_dtype, a1=None, bias=None, bias2=None, res=None):
-    """The lb_gemm mode flags of the element types: fp16 operands (0), or bf16 operands (LB_GEMM_BF16) with a bf16 or
-    (``out_dtype`` float16: LB_GEMM_OUT_F16) fp16 output.  Mixed operand types raise."""
-    if a0.dtype != torch.bfloat16 and w.dtype != torch.bfloat16:
-        return 0
-    _same_dtype(torch.bfloat16, "gemm operands a0 / w / a1 / bias / bias2 / res", a0, w, a1, bias, bias2, res)
-    if out_dtype == torch.bfloat16:
-        return _cabi.GEMM_BF16
-    if out_dtype == torch.float16:
-        return _cabi.GEMM_BF16 | _cabi.GEMM_OUT_F16
-    raise _cabi.LB200Error(f"gemm: bf16 operands give a bf16 or fp16 output (asked for {out_dtype})")
-
-
-_TILING = {"auto": 0, "box": _cabi.GEMM_TILE_BOX, "runs": _cabi.GEMM_TILE_RUNS}
+def _run1(dev, emit, t=0.0):
+    """Record one op with ``emit(P)`` into a fresh Program on device ``dev``, then finalize and run it."""
+    P = Program(dev)
+    emit(P)
+    P.finalize().run(t)
 
 
 def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None, out=None,
          mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto", out_dtype=None,
          depth_to_space=False):
-    """Tensor-core GEMM / implicit-GEMM conv (lb_gemm).  a0: NHWC activation viewed as
-    [B*H*W, >=a0_c] (row stride = a0.stride(0)); w: [N, K] packed weights.
-    ``tiling``: "auto" (the M tiling with fewer tiles), "box" (pixel boxes) or "runs" (pixel runs); all give the
-    same results.
-    Element types come from the tensors: fp16 throughout, or bf16 a0 / w / a1 / bias / bias2 / res (LB_GEMM_BF16)
-    with a bf16 output, or an fp16 one when ``out_dtype`` (default: ``out``'s dtype, else a0's) is torch.float16.
-    ``depth_to_space`` (LB_GEMM_D2S2): nearest-2x upsample + 3x3 conv of the H x W map a0, with ``w`` the [4*Co, 9*C]
-    phase weights (``taesd.pack_d2s_weights``); the output is the [B*2H*2W, Co] NHWC map."""
-    if tiling not in _TILING:
-        raise ValueError(f"tiling must be one of {sorted(_TILING)} (got {tiling!r})")
+    """Tensor-core GEMM / implicit-GEMM conv (``Program.gemm``).  The output (allocated unless ``out`` is given) is
+    [B*H*W, N] (N/2 with GEGLU, ``out_cols`` when given), or [B*2H*2W, N/4] with ``depth_to_space``, of type
+    ``out_dtype`` (default: ``out``'s, else a0's)."""
     dev = _dev(a0)
     M = B * H * W
-    a0_c = a0.shape[-1] if a0_c is None else a0_c
     n_out = (N // 2 if mode == 1 else N) if out_cols is None else out_cols
     if out_dtype is None:
         out_dtype = out.dtype if out is not None else a0.dtype
     elif out is not None and out.dtype != out_dtype:
         raise _cabi.LB200Error(f"gemm: out is {out.dtype}, out_dtype {out_dtype}")
-    dmode = gemm_dtype_mode(a0, w, out_dtype, a1, bias, bias2, res)
-    if depth_to_space:
-        dmode |= _cabi.GEMM_D2S2
     if out is None:
         shape = (4 * M, N // 4) if depth_to_space else (M, n_out)
         out = torch.empty(shape, dtype=out_dtype, device=a0.device)
-    d = _cabi.GemmDesc()
-    d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(-2), a0_c
-    if a1 is not None:
-        d.a1, d.a1_ld, d.a1_c = _p(a1), a1.stride(-2), (a1.shape[-1] if a1_c is None else a1_c)
-    d.B, d.H, d.W, d.taps = B, H, W, taps
-    d.w, d.w_ld, d.N = _p(w), w.stride(0), N
-    d.bias = _p(bias)
-    if bias2 is not None:
-        d.bias2, d.bias2_ld = _p(bias2), bias2.stride(0)
-    if res is not None:
-        d.res, d.res_ld = _p(res), res.stride(-2)
-    d.out, d.out_ld = _p(out), out.stride(-2)
-    d.mode = mode | (_cabi.GEMM_STATIC_W if static_w else 0) | (_cabi.GEMM_RELU if relu else 0) | _TILING[tiling] | dmode
-    if ln is not None:
-        d.ln_stats, d.ln_parts = _p(ln["stats"]), ln["stats"].shape[1]
-        d.ln_csum, d.ln_bias, d.ln_eps = _p(ln["csum"]), _p(ln["bias"]), ln["eps"]
-    if stats_out is not None:
-        d.stats_out, d.stats_parts = _p(stats_out), stats_out.shape[1]
-    check(_cabi.load().lb_gemm(ctx(dev), d, stream_ptr()), "lb_gemm")
+    _run1(dev, lambda P: P.gemm(a0, w, N, B, H, W, out, taps=taps, a0_c=a0_c, a1=a1, a1_c=a1_c, bias=bias,
+                                bias2=bias2, res=res, mode=mode, static_w=static_w, relu=relu, ln=ln,
+                                stats_out=stats_out, tiling=tiling, depth_to_space=depth_to_space))
     return out
 
 
 def gemm_stats_parts(a0, w, N, B, H, W, **kw):
     """Per-row partial count of lb_gemm's stats_out for this problem (4 per N tile)."""
-    import ctypes
-    dev = _dev(a0)
-    d = _cabi.GemmDesc()
-    M = B * H * W
-    out = torch.empty((M, N), dtype=torch.float16, device=a0.device)
-    d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(-2), kw.get("a0_c") or a0.shape[-1]
-    d.B, d.H, d.W, d.taps = B, H, W, kw.get("taps", 1)
-    d.w, d.w_ld, d.N = _p(w), w.stride(0), N
-    d.out, d.out_ld, d.mode = _p(out), out.stride(-2), kw.get("mode", 0)
-    return int(_cabi.load().lb_gemm_stats_parts(ctx(dev), ctypes.byref(d)))
+    out = torch.empty((B * H * W, N), dtype=torch.float16, device=a0.device)
+    return Program(_dev(a0)).gemm_stats_parts(a0, w, N, B, H, W, out, **kw)
 
 
 def lpips_tap(feat_a, feat_b, lin_w, out_scalar, workspace, accumulate=False):
@@ -240,28 +179,17 @@ def error_flag(dev=0):
 
 def attention(q, k, v, out, B, heads, Sq, Skv, q_col0=0, k_col0=0, v_col0=0, scale=0.125):
     """q/k/v: 2-D row-major fp16 buffers whose column slices hold the heads (lb_attention)."""
-    dev = _dev(q)
-    d = _cabi.AttnDesc()
-    d.q, d.q_ld, d.q_col0 = _p(q), q.stride(0), q_col0
-    d.k, d.k_ld, d.k_col0 = _p(k), k.stride(0), k_col0
-    d.v, d.v_ld, d.v_col0 = _p(v), v.stride(0), v_col0
-    d.out, d.out_ld = _p(out), out.stride(0)
-    d.B, d.heads, d.Sq, d.Skv, d.head_dim, d.scale = B, heads, Sq, Skv, 64, scale
-    check(_cabi.load().lb_attention(ctx(dev), d, stream_ptr()), "lb_attention")
+    _run1(_dev(q), lambda P: P.attention(q, k, v, out, B, heads, Sq, Skv, q_col0, k_col0, v_col0, scale))
     return out
 
 
 def groupnorm(x, B, HW, C, groups, gamma, beta, eps, silu, out=None):
     """fp16 or bf16 (x, gamma, beta and out of one type)."""
     dev = _dev(x)
-    dt = dtype16(x, "groupnorm x")
     if out is None:
         out = torch.empty((B * HW, C), dtype=x.dtype, device=x.device)
-    _same_dtype(x.dtype, "groupnorm x / gamma / beta / out", gamma, beta, out)
-    lib = _cabi.load()
-    ws = _gn_workspace(dev, lib.lb_groupnorm_workspace_bytes(ctx(dev), B, HW, groups))
-    check(lib.lb_groupnorm_dt(ctx(dev), ptr(x), x.stride(0), B, HW, C, groups, ptr(gamma), ptr(beta), float(eps),
-                              int(silu), ptr(out), out.stride(0), ptr(ws), stream_ptr(), dt), "lb_groupnorm")
+    ws = _gn_workspace(dev, _cabi.load().lb_groupnorm_workspace_bytes(ctx(dev), B, HW, groups))
+    _run1(dev, lambda P: P.groupnorm(x, B, HW, C, groups, gamma, beta, float(eps), silu, out, ws))
     return out
 
 
@@ -270,8 +198,7 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     rows, C = x.shape
     if out is None:
         out = torch.empty((rows, C), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_layernorm(ctx(dev), ptr(x), x.stride(0), rows, C, ptr(gamma), ptr(beta), float(eps),
-                                    ptr(out), out.stride(0), stream_ptr()), "lb_layernorm")
+    _run1(dev, lambda P: P.layernorm(x, gamma, beta, float(eps), out))
     return out
 
 
@@ -280,39 +207,27 @@ def embed_inputs(t, text_embeds, time_ids, dim_t, dim_a):
     B, pooled = text_embeds.shape
     temb_in = torch.empty((B, dim_t), dtype=torch.float16, device=text_embeds.device)
     add_in = torch.empty((B, pooled + 6 * dim_a), dtype=torch.float16, device=text_embeds.device)
-    check(_cabi.load().lb_embed_inputs(ctx(dev), float(t), ptr(text_embeds), ptr(time_ids), B, dim_t, pooled, dim_a,
-                                       ptr(temb_in), ptr(add_in), stream_ptr()), "lb_embed_inputs")
+    _run1(dev, lambda P: P.embed_inputs(text_embeds, time_ids, dim_t, dim_a, temb_in, add_in), t)
     return temb_in, add_in
 
 
 def linear_small(x, w, bias=None, addend=None, act_in=0, act_out=0, out=None):
     dev = _dev(x)
-    M, K = x.shape
-    N = w.shape[0]
+    M, _ = x.shape
     if out is None:
-        out = torch.empty((M, N), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_linear_small(ctx(dev), ptr(x), x.stride(0), M, K, ptr(w), w.stride(0), ptr(bias),
-                                       ptr(addend), 0 if addend is None else addend.stride(0), act_in, act_out,
-                                       ptr(out), out.stride(0), N, stream_ptr()), "lb_linear_small")
+        out = torch.empty((M, w.shape[0]), dtype=torch.float16, device=x.device)
+    _run1(dev, lambda P: P.linear_small(x, w, out, bias=bias, addend=addend, act_in=act_in, act_out=act_out))
     return out
 
 
-def conv_in(x_nchw, w_packed, bias, Cout, out=None, act=0, in_scale=1.0):
+def conv_in(x_nchw, w_packed, bias, Cout, out=None, act=_cabi.CONV_IN_PLAIN, in_scale=1.0):
     """fp16 or bf16 (x, weights, bias and out of one type).  ``act`` 1 (fp16): the tiny VAE decoder's input stage,
-    tanh(x * in_scale / 3) * 3 before the conv and ReLU after it (lb_conv_in_act)."""
+    tanh(x * in_scale / 3) * 3 before the conv and ReLU after it."""
     dev = _dev(x_nchw)
-    dt = dtype16(x_nchw, "conv_in x")
-    B, Cin, H, W = x_nchw.shape
+    B, _, H, W = x_nchw.shape
     if out is None:
         out = torch.empty((B * H * W, Cout), dtype=x_nchw.dtype, device=x_nchw.device)
-    _same_dtype(x_nchw.dtype, "conv_in x / w / bias / out", w_packed, bias, out)
-    if act:
-        check(_cabi.load().lb_conv_in_act(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout,
-                                          ptr(out), out.stride(0), int(act), float(in_scale), stream_ptr(), dt),
-              "lb_conv_in_act")
-        return out
-    check(_cabi.load().lb_conv_in_dt(ctx(dev), ptr(x_nchw), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout, ptr(out),
-                                     out.stride(0), stream_ptr(), dt), "lb_conv_in")
+    _run1(dev, lambda P: P.conv_in(x_nchw, w_packed, bias, Cout, out, act, in_scale))
     return out
 
 
@@ -320,30 +235,21 @@ def conv_out(x, B, H, W, Cin, w_packed, bias, Cout, out=None):
     dev = _dev(x)
     if out is None:
         out = torch.empty((B, Cout, H, W), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_conv_out(ctx(dev), ptr(x), x.stride(0), B, Cin, H, W, ptr(w_packed), ptr(bias), Cout,
-                                   ptr(out), stream_ptr()), "lb_conv_out")
+    _run1(dev, lambda P: P.conv_out(x, B, H, W, Cin, w_packed, bias, Cout, out))
     return out
 
 
 def upsample2x(x, B, H, W, C, out=None):
-    dev = _dev(x)
-    if out is None:
-        out = torch.empty((B * 4 * H * W, C), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_upsample2x(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), out.stride(0),
-                                     stream_ptr()), "lb_upsample2x")
-    return out
+    return upsample_nearest(x, B, H, W, C, 2 * H, 2 * W, out=out)
 
 
 def upsample_nearest(x, B, H, W, C, Ho, Wo, out=None):
     """F.interpolate(size=(Ho, Wo), mode="nearest") of NHWC rows [B*H*W, >=C] for Ho in {2H-1, 2H}, Wo in
     {2W-1, 2W} (lb_upsample_nearest; other sizes raise LB200Error)."""
     dev = _dev(x)
-    dt = dtype16(x, "upsample x")
     if out is None:
         out = torch.empty((B * Ho * Wo, C), dtype=x.dtype, device=x.device)
-    _same_dtype(x.dtype, "upsample x / out", out)
-    check(_cabi.load().lb_upsample_nearest_dt(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), out.stride(0),
-                                              Ho, Wo, stream_ptr(), dt), "lb_upsample_nearest")
+    _run1(dev, lambda P: P.upsample_nearest(x, B, H, W, C, out, Ho, Wo))
     return out
 
 
@@ -352,23 +258,20 @@ def im2col_s2(x, B, H, W, C, out=None):
     Ho, Wo = (H + 1) // 2, (W + 1) // 2
     if out is None:
         out = torch.empty((B * Ho * Wo, 9 * C), dtype=torch.float16, device=x.device)
-    check(_cabi.load().lb_im2col_s2(ctx(dev), ptr(x), x.stride(0), B, H, W, C, ptr(out), stream_ptr()),
-          "lb_im2col_s2")
+    _run1(dev, lambda P: P.im2col_s2(x, B, H, W, C, out))
     return out
 
 
-# ---- VAE-decoder helpers (fp16 or bf16; the decoder itself records them into a Program) ---------------------------
+# ---- VAE-decoder helpers (fp16 or bf16) ---------------------------------------------------------------------------
 
 
 def latent_prep(x_nchw, w_f32, bias_f32, out_dtype=torch.float16, out=None):
     """post_quant_conv(latents / scaling_factor): fp16 NCHW latents in, ``out_dtype`` (fp16 / bf16) NCHW out."""
     dev = _dev(x_nchw)
     assert x_nchw.dtype == torch.float16 and x_nchw.is_contiguous()
-    B, C, H, W = x_nchw.shape
     if out is None:
-        out = torch.empty((B, C, H, W), dtype=out_dtype, device=x_nchw.device)
-    check(_cabi.load().lb_latent_prep_dt(ctx(dev), ptr(x_nchw), B, C, H * W, ptr(w_f32), ptr(bias_f32), ptr(out),
-                                         stream_ptr(), dtype16(out, "latent_prep out")), "lb_latent_prep")
+        out = torch.empty(x_nchw.shape, dtype=out_dtype, device=x_nchw.device)
+    _run1(dev, lambda P: P.latent_prep(x_nchw, w_f32, bias_f32, out))
     return out
 
 
@@ -378,8 +281,7 @@ def softmax_rows(x, out=None, out_dtype=None):
     assert x.dtype == torch.float16
     if out is None:
         out = torch.empty(x.shape, dtype=out_dtype or x.dtype, device=x.device)
-    check(_cabi.load().lb_softmax_rows_dt(ctx(dev), ptr(x), x.stride(0), x.shape[0], x.shape[1], ptr(out),
-                                          out.stride(0), stream_ptr(), dtype16(out, "softmax out")), "lb_softmax_rows")
+    _run1(dev, lambda P: P.softmax_rows(x, out))
     return out
 
 
@@ -390,8 +292,7 @@ def postprocess_u8(img_nchw, out=None, nonfinite=None):
     B, C, H, W = img_nchw.shape
     if out is None:
         out = torch.empty((B, H, W, C), dtype=torch.uint8, device=img_nchw.device)
-    check(_cabi.load().lb_postprocess_u8_dt(ctx(dev), ptr(img_nchw), B, C, H * W, ptr(out), ptr(nonfinite),
-                                            stream_ptr(), dtype16(img_nchw, "postprocess image")), "lb_postprocess_u8")
+    _run1(dev, lambda P: P.postprocess_u8(img_nchw, out, nonfinite))
     return out
 
 
@@ -400,7 +301,5 @@ def nhwc_to_nchw(x, B, C, H, W, out=None):
     dev = _dev(x)
     if out is None:
         out = torch.empty((B, C, H, W), dtype=x.dtype, device=x.device)
-    _same_dtype(x.dtype, "nhwc_to_nchw x / out", out)
-    check(_cabi.load().lb_nhwc_to_nchw_dt(ctx(dev), ptr(x), x.stride(0), B, C, H * W, ptr(out), stream_ptr(),
-                                          dtype16(x, "nhwc_to_nchw x")), "lb_nhwc_to_nchw")
+    _run1(dev, lambda P: P.nhwc_to_nchw(x, B, C, H, W, out))
     return out

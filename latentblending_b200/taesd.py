@@ -11,7 +11,7 @@ scaling_factor)``, which for diffusers 0.25.0 ``DecoderTiny`` is
     return layers(x) * 2 - 1
 
 About 0.56 TFLOP per 1024^2 frame against the KL decoder's 10.5.  Lowering (fp16 storage, fp32 accumulation):
-  * the clamp, conv_in and its ReLU: one lb_conv_in_act (act 1) launch;
+  * the clamp, conv_in and its ReLU: one lb_conv_in (act 1) launch;
   * every block conv: an implicit-GEMM 3x3 conv with LB_GEMM_RELU; the third also adds the block input as the
     GEMM residual (bias, then residual, then ReLU: the reference's order), written over that input in place;
   * upsample + conv: ONE GEMM over the low-resolution map (LB_GEMM_D2S2) with four phase filters, whose epilogue
@@ -24,7 +24,8 @@ Activations ping-pong between three [pixels, C] buffers sized for the output res
 import torch
 
 from . import _cabi
-from .unet import Program, pack_conv_out8
+from .lowering import pack3
+from .program import Program, pack_conv_out8
 from .vae import DecoderBase
 
 DEFAULT_CONFIG = dict(latent_channels=4, out_channels=3, decoder_block_out_channels=(64, 64, 64, 64),
@@ -129,11 +130,6 @@ def pack_d2s_weights(w):
     return out.reshape(4 * Co, Ci, 3, 3)
 
 
-def _pack3(w):
-    """[N, Ci, 3, 3] -> the GEMM's [N][ky][kx][Ci] rows."""
-    return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
-
-
 class TinyVAEDecoderB200(DecoderBase):
     """The AutoencoderTiny decoder, fp16 storage / fp32 accumulation (the only precision it has here)."""
     dtype = torch.float16
@@ -162,10 +158,10 @@ class TinyVAEDecoderB200(DecoderBase):
                 W["in.b"] = f16(f32(f"layers.{idx}.bias"))
             elif kind == "block":
                 for j in (0, 2, 4):
-                    W[f"{idx}.{j}.w"] = f16(_pack3(f32(f"layers.{idx}.conv.{j}.weight")))
+                    W[f"{idx}.{j}.w"] = f16(pack3(f32(f"layers.{idx}.conv.{j}.weight")))
                     W[f"{idx}.{j}.b"] = f16(f32(f"layers.{idx}.conv.{j}.bias"))
             elif kind == "up_conv":
-                W[f"{idx}.w"] = f16(_pack3(pack_d2s_weights(f32(f"layers.{idx}.weight"))))
+                W[f"{idx}.w"] = f16(pack3(pack_d2s_weights(f32(f"layers.{idx}.weight"))))
             else:
                 # decode() returns layers(x) * 2 - 1: folded into the last conv in fp32
                 w = f32(f"layers.{idx}.weight") * 2.0
@@ -191,8 +187,8 @@ class _TinyLowering:
         self.frame = torch.zeros(Ho, Wo, 3, dtype=torch.uint8, device=dev)
         bufs = [torch.empty(Ho * Wo, C, **f16) for _ in range(3)]
         xi, hh, ww = 0, h, w
-        P.conv_in_act(self.z_in, Wt["in.w"], Wt["in.b"], C, bufs[xi][: h * w], _cabi.CONV_IN_TINY_VAE,
-                      1.0 / vae.scaling_factor)
+        P.conv_in(self.z_in, Wt["in.w"], Wt["in.b"], C, bufs[xi][: h * w], _cabi.CONV_IN_TINY_VAE,
+                  1.0 / vae.scaling_factor)
         for kind, idx, _ in vae.layout[1:]:
             M = hh * ww
             x = bufs[xi][:M]

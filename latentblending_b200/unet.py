@@ -19,18 +19,15 @@ Data layout in HBM (all fp16):
     all resnet ``time_emb_proj`` stacked into one [sum Cout, T] matrix.
   * latents / eps stay NCHW [B,4,h,w] like the reference's tensors.
 """
-import ctypes
-import os
 from dataclasses import dataclass
 from typing import Tuple
 
 import torch
 
 from . import _cabi
-from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_CONV_OUT, OP_EMBED_INPUTS, OP_GEMM,
-                    OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
-                    OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS, OP_UPSAMPLE2X, Op, check, ctx,
-                    stream_ptr)
+from ._cabi import ctx
+from .lowering import Scratch, lower_conv_out, lower_resnet, pack3, pack_resnet
+from .program import Program, pack_conv_out8
 
 
 @dataclass
@@ -55,264 +52,6 @@ class UNetConfig:
     @property
     def add_in_dim(self):
         return self.pooled_dim + 6 * self.addition_time_embed_dim
-
-
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
-class Program:
-    """A recorded op list; ``finalize`` hands it to lb_program_create."""
-
-    def __init__(self, device_index):
-        self.dev = device_index
-        self.ops = []
-        self.keep = []          # tensors referenced by raw pointers must outlive the program
-        self.handle = None
-
-    def _new(self, kind):
-        op = Op()
-        op.kind = kind
-        self.ops.append(op)
-        return op
-
-    def hold(self, *ts):
-        self.keep.extend(t for t in ts if t is not None)
-
-    # -- op emitters (mirror latentblending_b200.ops, but record instead of launching) --------
-    def gemm(self, a0, w, N, B, H, W, out, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None,
-             mode=0, static_w=True, relu=False, ln=None, stats_out=None, depth_to_space=False):
-        """``static_w``: ``w`` holds model weights (not written by the preceding op), so the kernel may fetch its
-        first tiles before the preceding kernel has finished (LB_GEMM_STATIC_W).  Pass False when an activation
-        is used as the B operand.
-        ``depth_to_space``: nearest-2x upsample + 3x3 conv as one GEMM (LB_GEMM_D2S2): ``w`` holds the four phase
-        filters [4*Co, 9*C], ``out`` the [B*2H*2W, Co] upsampled map.
-        ``ln``: dict(stats=[M,parts,2] fp32, csum=[N] fp32, bias=[N] fp32, eps) -- LayerNorm folded into this GEMM
-        (``w`` must already hold w*gamma; see include/lb200.h).  ``stats_out``: [M,parts,2] fp32 buffer that receives
-        this GEMM's per-row partial sums for a following LN-folded GEMM (parts = self.gemm_stats_parts(...)).
-        Element types come from the tensors as in ``ops.gemm``: bf16 operands (LB_GEMM_BF16) write ``out``'s type."""
-        from .ops import gemm_dtype_mode
-        dmode = gemm_dtype_mode(a0, w, out.dtype, a1, bias, bias2, res)
-        d = self._new(OP_GEMM).u.gemm
-        d.a0, d.a0_ld, d.a0_c = _p(a0), a0.stride(0), (a0.shape[1] if a0_c is None else a0_c)
-        if a1 is not None:
-            d.a1, d.a1_ld, d.a1_c = _p(a1), a1.stride(0), (a1.shape[1] if a1_c is None else a1_c)
-        d.B, d.H, d.W, d.taps = B, H, W, taps
-        d.w, d.w_ld, d.N = _p(w), w.stride(0), N
-        d.bias = _p(bias)
-        if bias2 is not None:
-            d.bias2, d.bias2_ld = _p(bias2), bias2.stride(0)
-        if res is not None:
-            d.res, d.res_ld = _p(res), res.stride(0)
-        d.out, d.out_ld = _p(out), out.stride(0)
-        d.mode = mode | (GEMM_STATIC_W if static_w else 0) | (GEMM_RELU if relu else 0) | dmode
-        if depth_to_space:
-            d.mode |= _cabi.GEMM_D2S2
-        if ln is not None:
-            st = ln["stats"]
-            assert st.dtype == torch.float32 and st.dim() == 3 and st.shape[2] == 2 and st.is_contiguous()
-            d.ln_stats, d.ln_parts = _p(st), st.shape[1]
-            d.ln_csum, d.ln_bias, d.ln_eps = _p(ln["csum"]), _p(ln["bias"]), ln["eps"]
-            self.hold(st, ln["csum"], ln["bias"])
-        if stats_out is not None:
-            assert stats_out.dtype == torch.float32 and stats_out.dim() == 3 and stats_out.is_contiguous()
-            d.stats_out, d.stats_parts = _p(stats_out), stats_out.shape[1]
-            self.hold(stats_out)
-        self.hold(a0, w, a1, bias, bias2, res, out)
-
-    def gemm_stats_parts(self, a0, w, N, B, H, W, out, **kw):
-        """Number of per-row partials a GEMM with these arguments writes through ``stats_out``."""
-        probe = Program(self.dev)
-        probe.gemm(a0, w, N, B, H, W, out, **kw)
-        n = int(_cabi.load().lb_gemm_stats_parts(ctx(self.dev), ctypes.byref(probe.ops[0].u.gemm)))
-        if n < 0:
-            raise _cabi.LB200Error("lb_gemm_stats_parts failed: " + _cabi.load().lb_last_error().decode())
-        return n
-
-    def lpips_im2col_u8(self, frame_u8, H, W, k, stride, pad, shift, scale, out):
-        d = self._new(OP_LPIPS_IM2COL_U8).u.patch
-        d.x, d.H, d.W, d.C, d.k, d.stride, d.pad = _p(frame_u8), H, W, out.shape[1], k, stride, pad
-        d.out, d.ld_out = _p(out), out.stride(0)
-        for i in range(3):
-            d.f[i], d.f[3 + i] = shift[i], scale[i]
-        self.hold(frame_u8, out)
-
-    def im2col(self, x, H, W, C, k, stride, pad, out):
-        d = self._new(OP_IM2COL).u.patch
-        d.x, d.ld_x, d.H, d.W, d.C, d.k, d.stride, d.pad = _p(x), x.stride(0), H, W, C, k, stride, pad
-        d.out, d.ld_out = _p(out), out.stride(0)
-        self.hold(x, out)
-
-    def maxpool3s2(self, x, H, W, C, out):
-        d = self._new(OP_MAXPOOL3S2).u.patch
-        d.x, d.ld_x, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), H, W, C, _p(out), out.stride(0)
-        self.hold(x, out)
-
-    def attention(self, q, k, v, out, B, heads, Sq, Skv, q_col0=0, k_col0=0, v_col0=0, scale=0.125):
-        d = self._new(OP_ATTENTION).u.attn
-        d.q, d.q_ld, d.q_col0 = _p(q), q.stride(0), q_col0
-        d.k, d.k_ld, d.k_col0 = _p(k), k.stride(0), k_col0
-        d.v, d.v_ld, d.v_col0 = _p(v), v.stride(0), v_col0
-        d.out, d.out_ld = _p(out), out.stride(0)
-        d.B, d.heads, d.Sq, d.Skv, d.head_dim, d.scale = B, heads, Sq, Skv, 64, scale
-        self.hold(q, k, v, out)
-
-    # The VAE-decoder builders below take ``dtype`` (LB_DTYPE_F16 = 0 / LB_DTYPE_BF16 = 1): the lb_op.dtype of the
-    # record, i.e. the element type of their 16-bit tensors (see include/lb200.h for each op's meaning).
-    def _new_dt(self, kind, dtype):
-        op = self._new(kind)
-        op.dtype = dtype
-        return op
-
-    def groupnorm(self, x, B, HW, C, groups, gamma, beta, eps, silu, out, ws, dtype=0):
-        d = self._new_dt(OP_GROUPNORM, dtype).u.norm
-        d.x, d.ld_x, d.rows, d.B, d.C, d.groups, d.silu, d.eps = _p(x), x.stride(0), HW, B, C, groups, int(silu), eps
-        d.gamma, d.beta, d.out, d.ld_out, d.workspace = _p(gamma), _p(beta), _p(out), out.stride(0), _p(ws)
-        self.hold(x, gamma, beta, out, ws)
-
-    def layernorm(self, x, gamma, beta, eps, out):
-        d = self._new(OP_LAYERNORM).u.norm
-        d.x, d.ld_x, d.rows, d.B, d.C, d.eps = _p(x), x.stride(0), x.shape[0], 1, x.shape[1], eps
-        d.gamma, d.beta, d.out, d.ld_out = _p(gamma), _p(beta), _p(out), out.stride(0)
-        self.hold(x, gamma, beta, out)
-
-    def embed_inputs(self, text_embeds, time_ids, dim_t, dim_a, temb_in, add_in):
-        d = self._new(OP_EMBED_INPUTS).u.embed
-        d.text_embeds, d.time_ids = _p(text_embeds), _p(time_ids)
-        d.B, d.dim_t, d.pooled, d.dim_a = text_embeds.shape[0], dim_t, text_embeds.shape[1], dim_a
-        d.temb_in, d.add_in = _p(temb_in), _p(add_in)
-        self.hold(text_embeds, time_ids, temb_in, add_in)
-
-    def linear_small(self, x, w, out, bias=None, addend=None, act_in=0, act_out=0):
-        d = self._new(OP_LINEAR_SMALL).u.lin
-        d.x, d.ldx, d.M, d.K = _p(x), x.stride(0), x.shape[0], x.shape[1]
-        d.w, d.ldw, d.bias = _p(w), w.stride(0), _p(bias)
-        if addend is not None:
-            d.addend, d.ldadd = _p(addend), addend.stride(0)
-        d.act_in, d.act_out, d.out, d.ldo, d.N = act_in, act_out, _p(out), out.stride(0), w.shape[0]
-        self.hold(x, w, out, bias, addend)
-
-    def conv_in(self, x_nchw, w, bias, Cout, out, dtype=0):
-        d = self._new_dt(OP_CONV_IN, dtype).u.conv
-        B, Cin, H, W = x_nchw.shape
-        d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
-        d.out, d.ld_out = _p(out), out.stride(0)
-        self.hold(x_nchw, w, bias, out)
-
-    def conv_in_act(self, x_nchw, w, bias, Cout, out, act, in_scale=1.0, dtype=0):
-        """lb_conv_in_act: ``act`` 1 is the tiny VAE decoder's input stage (tanh clamp, conv, ReLU)."""
-        d = self._new_dt(_cabi.OP_CONV_IN_ACT, dtype).u.conv_act
-        B, Cin, H, W = x_nchw.shape
-        d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
-        d.out, d.ld_out, d.act, d.in_scale = _p(out), out.stride(0), act, in_scale
-        self.hold(x_nchw, w, bias, out)
-
-    def conv_out(self, x, B, H, W, Cin, w, bias, Cout, out_nchw):
-        d = self._new(OP_CONV_OUT).u.conv
-        d.x, d.ld_x, d.B, d.Cin, d.H, d.W = _p(x), x.stride(0), B, Cin, H, W
-        d.w, d.bias, d.Cout, d.out = _p(w), _p(bias), Cout, _p(out_nchw)
-        self.hold(x, w, bias, out_nchw)
-
-    def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp, dtype=0):
-        """The C0 -> Cout (<= 8) 3x3 output convolution on the tensor-core GEMM: N = 8 (zero-padded weight rows),
-        then the Cout live columns go back to NCHW.  ``tmp``: [B*H*W, 8] scratch of the decoder's type."""
-        self.gemm(x, w8, 8, B, H, W, tmp, taps=9, a0_c=Cin, bias=bias8)
-        d = self._new_dt(OP_NHWC_TO_NCHW, dtype).u.aux
-        d.x, d.ld_x, d.out, d.n, d.B, d.C = _p(tmp), tmp.stride(0), _p(out_nchw), H * W, B, Cout
-        self.hold(tmp, out_nchw)
-
-    def upsample2x(self, x, B, H, W, C, out, Ho=0, Wo=0, dtype=0):
-        """Nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}; 0 = exactly 2x)."""
-        d = self._new_dt(OP_UPSAMPLE2X, dtype).u.resample
-        d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
-        d.Ho, d.Wo = Ho, Wo
-        self.hold(x, out)
-
-    def im2col_s2(self, x, B, H, W, C, out):
-        d = self._new(OP_IM2COL_S2).u.resample
-        d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
-        self.hold(x, out)
-
-    def latent_prep(self, x_nchw, w_f32, bias_f32, out_nchw, dtype=0):
-        d = self._new_dt(OP_LATENT_PREP, dtype).u.aux
-        B, C, H, W = x_nchw.shape
-        d.x, d.w, d.bias, d.out, d.n, d.B, d.C = _p(x_nchw), _p(w_f32), _p(bias_f32), _p(out_nchw), H * W, B, C
-        self.hold(x_nchw, w_f32, bias_f32, out_nchw)
-
-    def softmax_rows(self, x, out, dtype=0):
-        """fp16 rows in; ``dtype``: the output's type (may write over ``x``, see lb_softmax_rows_dt)."""
-        d = self._new_dt(OP_SOFTMAX_ROWS, dtype).u.aux
-        d.x, d.ld_x, d.out, d.ld_out, d.n, d.C = _p(x), x.stride(0), _p(out), out.stride(0), x.shape[0], x.shape[1]
-        self.hold(x, out)
-
-    def postprocess_u8(self, img_nchw, out_u8, nonfinite=None, dtype=0):
-        d = self._new_dt(OP_POSTPROCESS_U8, dtype).u.aux
-        B, C, H, W = img_nchw.shape
-        d.x, d.out, d.n, d.B, d.C, d.w = _p(img_nchw), _p(out_u8), H * W, B, C, _p(nonfinite)
-        self.hold(img_nchw, out_u8, nonfinite)
-
-    # -- lifecycle --------------------------------------------------------------------------
-    def finalize(self):
-        arr = (Op * len(self.ops))(*self.ops)
-        h = ctypes.c_void_p()
-        check(_cabi.load().lb_program_create(ctx(self.dev), arr, len(self.ops), ctypes.byref(h)), "lb_program_create")
-        self.handle = h
-        self.num_launches = int(_cabi.load().lb_program_num_launches(h))
-        return self
-
-    def run(self, t=0.0):
-        check(_cabi.load().lb_program_run(self.handle, float(t), stream_ptr()), "lb_program_run")
-        from . import ops
-        ops.LAUNCHES[0] += self.num_launches
-
-    def run_kinds(self, kinds, t=0.0):
-        """Profiling aid: replay only ops of the given kinds (e.g. [OP_GEMM])."""
-        mask = 0
-        for k in kinds:
-            mask |= 1 << k
-        check(_cabi.load().lb_program_run_kinds(self.handle, float(t), mask, stream_ptr()), "lb_program_run_kinds")
-        return int(_cabi.load().lb_program_count_kinds(self.handle, mask))
-
-    def work(self):
-        """Algorithmic work of the recorded ops: {'gemm_flops', 'gemm_bytes', 'attn_flops', 'norm_bytes'}.
-        gemm_bytes = fp16 bytes every GEMM must move at least once: A (M x C per input tensor -- a 3x3 conv reads its
-        activation once), W (N x K), the output and the residual."""
-        gemm = attn = norm = gbytes = 0
-        for op in self.ops:
-            if op.kind == OP_GEMM:
-                d = op.u.gemm
-                M, K = d.B * d.H * d.W, d.taps * d.a0_c + (d.a1_c if d.a1 else 0)
-                gemm += 2 * M * d.N * K
-                n_out = d.N // 2 if (d.mode & 0xff) == 1 else d.N
-                gbytes += 2 * (M * (d.a0_c + (d.a1_c if d.a1 else 0)) + d.N * K + M * n_out + (M * d.N if d.res else 0))
-            elif op.kind == OP_ATTENTION:
-                d = op.u.attn
-                attn += 4 * d.B * d.heads * d.Sq * d.Skv * d.head_dim
-            elif op.kind in (OP_GROUPNORM, OP_LAYERNORM):
-                d = op.u.norm
-                rows = d.rows * (d.B if op.kind == OP_GROUPNORM else 1)
-                norm += 4 * rows * d.C
-        return dict(gemm_flops=gemm, gemm_bytes=gbytes, attn_flops=attn, norm_bytes=norm)
-
-    def __del__(self):
-        try:
-            if self.handle is not None:
-                _cabi.load().lb_program_destroy(self.handle)
-        except Exception:
-            pass
-
-
-def pack_conv_out8(w_co_ky_kx_ci, bias):
-    """[Cout<=8][3][3][Cin] conv_out weights -> ([8, 9*Cin] zero-padded rows, [8] bias) for the N = 8 GEMM; None when
-    Cin is not a multiple of 64 (the GEMM's K blocks) -- the direct lb_conv_out kernel is used then."""
-    co, cin = w_co_ky_kx_ci.shape[0], w_co_ky_kx_ci.shape[-1]
-    if cin % 64 != 0 or co > 8:
-        return None, None
-    w8 = torch.zeros(8, 9 * cin, dtype=w_co_ky_kx_ci.dtype, device=w_co_ky_kx_ci.device)     # fp16, or bf16
-    w8[:co] = w_co_ky_kx_ci.reshape(co, 9 * cin)
-    b8 = torch.zeros(8, dtype=bias.dtype, device=bias.device)
-    b8[:co] = bias
-    return w8.contiguous(), b8.contiguous()
 
 
 def _fold_layernorm(w, bias, gamma, beta):
@@ -344,10 +83,6 @@ class PackedUNet:
         def g(name):
             return sd[name].detach().to(device=dev, dtype=torch.float16).contiguous()
 
-        def conv3(name):      # [Cout,Cin,3,3] -> [Cout][ky][kx][Cin]
-            w = g(name + ".weight")
-            return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
-
         self.g = g
         self.w = {}
         W = self.w
@@ -366,16 +101,7 @@ class PackedUNet:
         temb_w, temb_b, off = [], [], 0
         self.temb_off = {}
         for r in self.resnet_names:
-            W[r + ".norm1.g"], W[r + ".norm1.b"] = g(r + ".norm1.weight"), g(r + ".norm1.bias")
-            W[r + ".norm2.g"], W[r + ".norm2.b"] = g(r + ".norm2.weight"), g(r + ".norm2.bias")
-            W[r + ".conv1.w"], W[r + ".conv1.b"] = conv3(r + ".conv1"), g(r + ".conv1.bias")
-            w2, b2 = conv3(r + ".conv2"), g(r + ".conv2.bias")
-            if (r + ".conv_shortcut.weight") in sd:
-                ws = g(r + ".conv_shortcut.weight")
-                w2 = torch.cat([w2, ws.reshape(ws.shape[0], -1)], dim=1).contiguous()
-                b2 = (b2.float() + g(r + ".conv_shortcut.bias").float()).half()
-                W[r + ".has_shortcut"] = True
-            W[r + ".conv2.w"], W[r + ".conv2.b"] = w2, b2
+            pack_resnet(W, r, sd, g)
             tw, tb = g(r + ".time_emb_proj.weight"), g(r + ".time_emb_proj.bias")
             self.temb_off[r] = (off, tw.shape[0])
             off += tw.shape[0]
@@ -420,7 +146,7 @@ class PackedUNet:
         for k in sd:
             if k.endswith("samplers.0.conv.weight"):
                 nm = k[: -len(".weight")]
-                W[nm + ".w"], W[nm + ".b"] = conv3(nm), g(nm + ".bias")
+                W[nm + ".w"], W[nm + ".b"] = pack3(g(nm + ".weight")), g(nm + ".bias")
 
     def nbytes(self):
         return sum(t.numel() * t.element_size() for t in self.w.values() if torch.is_tensor(t))
@@ -492,16 +218,8 @@ class _Lowering:
                               dtype=torch.uint8, device=dev)
         P = self.prog_step = Program(net.dev_index)
         PC = self.prog_ctx = Program(net.dev_index)
-        self._scratch = {}
-
-        def scratch(name, rows, cols):
-            key = name
-            need = rows * cols
-            buf = self._scratch.get(key)
-            if buf is None or buf.numel() < need:
-                buf = torch.empty(need, **f16)
-                self._scratch[key] = buf
-            return buf[:need].view(rows, cols)
+        scratch = Scratch(torch.float16, dev)
+        ln_stats = {}
 
         self._persist = []
 
@@ -558,17 +276,7 @@ class _Lowering:
 
         def resnet(rname, x, cin, cout, level, out):
             h_, w_ = res_hw[level]
-            M = rows_at(level)
-            n1 = scratch("n1", M, cin)
-            P.groupnorm(x, B, h_ * w_, cin, groups, Wt[rname + ".norm1.g"], Wt[rname + ".norm1.b"], 1e-5, 1, n1, self.ws)
-            h1 = scratch("h1", M, cout)
-            P.gemm(n1, Wt[rname + ".conv1.w"], cout, B, h_, w_, h1, taps=9, bias=Wt[rname + ".conv1.b"], bias2=tslice(rname))
-            n2 = scratch("n2", M, cout)
-            P.groupnorm(h1, B, h_ * w_, cout, groups, Wt[rname + ".norm2.g"], Wt[rname + ".norm2.b"], 1e-5, 1, n2, self.ws)
-            if Wt.get(rname + ".has_shortcut"):
-                P.gemm(n2, Wt[rname + ".conv2.w"], cout, B, h_, w_, out, taps=9, a1=x, a1_c=cin, bias=Wt[rname + ".conv2.b"])
-            else:
-                P.gemm(n2, Wt[rname + ".conv2.w"], cout, B, h_, w_, out, taps=9, bias=Wt[rname + ".conv2.b"], res=x)
+            lower_resnet(P, Wt, rname, x, cin, cout, B, h_, w_, out, groups, 1e-5, self.ws, scratch, bias2=tslice(rname))
 
         kv_cache = {}
 
@@ -591,10 +299,9 @@ class _Lowering:
                 # every GEMM that writes the residual stream ``hs`` also writes its per-row partial sums; the three
                 # LayerNorms of a block are folded into the GEMMs that consume them (no LN launches, no LN buffer)
                 parts = P.gemm_stats_parts(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs)
-                key = ("ln_stats", M, parts)
-                if key not in self._scratch:
-                    self._scratch[key] = torch.zeros(M, parts, 2, **f32)
-                stats = self._scratch[key]
+                if (M, parts) not in ln_stats:
+                    ln_stats[(M, parts)] = torch.zeros(M, parts, 2, **f32)
+                stats = ln_stats[(M, parts)]
                 P.gemm(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs, bias=Wt[aname + ".proj_in.b"], stats_out=stats)
 
             def ln_of(t, key):
@@ -699,15 +406,11 @@ class _Lowering:
                 h_, w_ = res_hw[lvl]
                 ho, wo = res_hw[lvl - 1]
                 up = scratch("up", rows_at(lvl - 1), cout)
-                P.upsample2x(x, B, h_, w_, cout, up, ho, wo)
+                P.upsample_nearest(x, B, h_, w_, cout, up, ho, wo)
                 P.gemm(up, Wt[nm + ".w"], cout, B, ho, wo, cats[ci]["hidden"], taps=9, bias=Wt[nm + ".b"])
         # ---- out ----------------------------------------------------------------------------
         no = scratch("n1", rows_at(0), ch[0])
         P.groupnorm(x, B, H * W, ch[0], groups, Wt["conv_norm_out.g"], Wt["conv_norm_out.b"], 1e-5, 1, no, self.ws)
-        if Wt.get("conv_out.w8") is not None and os.environ.get("LB_CONV_OUT_DIRECT") is None:
-            P.conv_out_gemm(no, B, H, W, ch[0], Wt["conv_out.w8"], Wt["conv_out.b8"], cfg.out_channels, self.eps,
-                            scratch("conv_out8", rows_at(0), 8))
-        else:
-            P.conv_out(no, B, H, W, ch[0], Wt["conv_out.w"], Wt["conv_out.b"], cfg.out_channels, self.eps)
+        lower_conv_out(P, Wt, no, B, H, W, ch[0], cfg.out_channels, self.eps, scratch)
         P.finalize()
         PC.finalize()

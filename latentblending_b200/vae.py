@@ -12,16 +12,12 @@ scores = (Wq x)(Wk x)^T (1/sqrt(C) folded into Wq), P = softmax_rows(scores), ou
 produced directly by a GEMM with swapped operands; the value bias is folded into the output bias
 (softmax rows sum to one).  Weights use the diffusers state_dict names.
 """
-import os
-
 import torch
 
 from . import _cabi
 from ._cabi import ctx
-from .unet import Program, pack_conv_out8
-
-
-_DTYPES = {torch.float16: _cabi.DTYPE_F16, torch.bfloat16: _cabi.DTYPE_BF16}
+from .lowering import Scratch, lower_conv_out, lower_resnet, pack3, pack_resnet
+from .program import Program, pack_conv_out8
 
 
 class DecoderBase:
@@ -72,14 +68,13 @@ class VAEDecoderB200(DecoderBase):
     def __init__(self, state_dict, channels, scaling_factor, device, groups=32, dtype=torch.float16):
         """``dtype``: torch.float16 or torch.bfloat16, the storage type of weights and activations (fp32 accumulation
         either way).  Weights are cast once from the state dict's own dtype; folded biases are formed in fp32."""
-        if dtype not in _DTYPES:
+        if dtype not in (torch.float16, torch.bfloat16):
             raise ValueError(f"VAE decoder dtype must be torch.float16 or torch.bfloat16 (got {dtype})")
         super().__init__(device)
         self.channels = tuple(channels)
         self.scaling_factor = scaling_factor
         self.groups = groups
         self.dtype = dtype
-        self.lb_dtype = _DTYPES[dtype]
         sd = state_dict
         dev = self.device
 
@@ -88,10 +83,6 @@ class VAEDecoderB200(DecoderBase):
 
         def gf(n):
             return sd[n].detach().to(device=dev, dtype=torch.float32)
-
-        def conv3(n):
-            w = g(n + ".weight")
-            return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1).contiguous()
 
         W = self.w = {}
         pq = gf("post_quant_conv.weight")
@@ -102,19 +93,7 @@ class VAEDecoderB200(DecoderBase):
         W["conv_in.b"] = g("conv_in.bias")
         self.resnets = [k[: -len(".norm1.weight")] for k in sd if k.endswith(".norm1.weight")]
         for r in self.resnets:
-            W[r + ".norm1.g"], W[r + ".norm1.b"] = g(r + ".norm1.weight"), g(r + ".norm1.bias")
-            W[r + ".norm2.g"], W[r + ".norm2.b"] = g(r + ".norm2.weight"), g(r + ".norm2.bias")
-            W[r + ".conv1.w"], W[r + ".conv1.b"] = conv3(r + ".conv1"), g(r + ".conv1.bias")
-            w2, b2 = conv3(r + ".conv2"), g(r + ".conv2.bias")
-            if (r + ".conv_shortcut.weight") in sd:
-                ws = g(r + ".conv_shortcut.weight")
-                w2 = torch.cat([w2, ws.reshape(ws.shape[0], -1)], 1).contiguous()
-                if dtype == torch.float16:
-                    b2 = (b2.float() + g(r + ".conv_shortcut.bias").float()).half()
-                else:
-                    b2 = (gf(r + ".conv2.bias") + gf(r + ".conv_shortcut.bias")).to(dtype)
-                W[r + ".has_shortcut"] = True
-            W[r + ".conv2.w"], W[r + ".conv2.b"] = w2, b2
+            pack_resnet(W, r, sd, g)
         a = "mid_block.attentions.0"
         Cm = sd[a + ".to_q.weight"].shape[0]
         scale = Cm ** -0.5
@@ -127,7 +106,7 @@ class VAEDecoderB200(DecoderBase):
         for k in sd:
             if k.endswith("upsamplers.0.conv.weight"):
                 nm = k[: -len(".weight")]
-                W[nm + ".w"], W[nm + ".b"] = conv3(nm), g(nm + ".bias")
+                W[nm + ".w"], W[nm + ".b"] = pack3(g(nm + ".weight")), g(nm + ".bias")
         W["norm_out.g"], W["norm_out.b"] = g("conv_norm_out.weight"), g("conv_norm_out.bias")
         W["conv_out.w"] = g("conv_out.weight").permute(0, 2, 3, 1).contiguous()
         W["conv_out.b"] = g("conv_out.bias")
@@ -152,8 +131,6 @@ class _VAELowering:
         Wt, dev, groups = vae.w, vae.device, vae.groups
         f16 = dict(dtype=torch.float16, device=dev)
         act = dict(dtype=vae.dtype, device=dev)       # activations and scratch: the decoder's type
-        dt = vae.lb_dtype
-        bf16 = vae.dtype == torch.bfloat16
         ch = list(reversed(vae.channels))            # e.g. [512, 512, 256, 128]
         B = 1
         P = self.prog = Program(vae.dev_index)
@@ -162,33 +139,17 @@ class _VAELowering:
         self.frame = torch.zeros(H, W_, 3, dtype=torch.uint8, device=dev)
         self.ws = torch.zeros(max(1 << 16, _cabi.load().lb_groupnorm_workspace_bytes(ctx(vae.dev_index), B, H * W_, groups)),
                               dtype=torch.uint8, device=dev)
-        scratch = {}
-
-        def sc(name, rows, cols):
-            need = rows * cols
-            if name not in scratch or scratch[name].numel() < need:
-                scratch[name] = torch.empty(need, **act)
-            return scratch[name][:need].view(rows, cols)
+        sc = Scratch(vae.dtype, dev)
 
         def resnet(rname, x, cin, cout, hh, ww, out):
-            M = hh * ww
-            n1 = sc("n1", M, cin)
-            P.groupnorm(x, B, M, cin, groups, Wt[rname + ".norm1.g"], Wt[rname + ".norm1.b"], 1e-6, 1, n1, self.ws, dt)
-            h1 = sc("h1", M, cout)
-            P.gemm(n1, Wt[rname + ".conv1.w"], cout, B, hh, ww, h1, taps=9, bias=Wt[rname + ".conv1.b"])
-            n2 = sc("n2", M, cout)
-            P.groupnorm(h1, B, M, cout, groups, Wt[rname + ".norm2.g"], Wt[rname + ".norm2.b"], 1e-6, 1, n2, self.ws, dt)
-            if Wt.get(rname + ".has_shortcut"):
-                P.gemm(n2, Wt[rname + ".conv2.w"], cout, B, hh, ww, out, taps=9, a1=x, a1_c=cin, bias=Wt[rname + ".conv2.b"])
-            else:
-                P.gemm(n2, Wt[rname + ".conv2.w"], cout, B, hh, ww, out, taps=9, bias=Wt[rname + ".conv2.b"], res=x)
+            lower_resnet(P, Wt, rname, x, cin, cout, B, hh, ww, out, groups, 1e-6, self.ws, sc)
 
         z = torch.empty(1, 4, h, w, **act)
-        P.latent_prep(self.z_in, Wt["prep.w"], Wt["prep.b"], z, dt)
+        P.latent_prep(self.z_in, Wt["prep.w"], Wt["prep.b"], z)
         C0 = ch[0]
         S = h * w
         x = torch.empty(S, C0, **act)
-        P.conv_in(z, Wt["conv_in.w"], Wt["conv_in.b"], C0, x, dt)
+        P.conv_in(z, Wt["conv_in.w"], Wt["conv_in.b"], C0, x)
         x2 = torch.empty(S, C0, **act)
         resnet("mid_block.resnets.0", x, C0, C0, h, w, x2)
         # mid-block attention (single head, dim C0)
@@ -196,7 +157,7 @@ class _VAELowering:
         # the extra ones zero (never written), so the extra V^T and score columns are exact zeros
         S8 = -(-S // 8) * 8
         hn = torch.zeros(S8, C0, **act)
-        P.groupnorm(x2, B, S, C0, groups, Wt["attn.norm.g"], Wt["attn.norm.b"], 1e-6, 0, hn, self.ws, dt)
+        P.groupnorm(x2, B, S, C0, groups, Wt["attn.norm.g"], Wt["attn.norm.b"], 1e-6, 0, hn, self.ws)
         qk = torch.zeros(S8, 2 * C0, **act)
         P.gemm(hn, Wt["attn.qk.w"], 2 * C0, 1, 1, S, qk, bias=Wt["attn.qk.b"])
         # P V contracts over the S keys, and the GEMM's K must be a multiple of 64: P and V^T get Sp >= S8 columns, the
@@ -210,7 +171,7 @@ class _VAELowering:
         # writes the bf16 P over them (same 2-byte slots), which P V reads as a bf16 operand
         P.gemm(qk[:, :C0], qk[:, C0:], S8, 1, 1, S, scores[:, :S8], static_w=False)      # (scaled q) k^T
         probs = scores.view(vae.dtype)
-        P.softmax_rows(scores[:, :S], probs[:, :S], dt)
+        P.softmax_rows(scores[:, :S], probs[:, :S])
         att = sc("h1", S, C0)
         P.gemm(probs, vT, C0, 1, 1, S, att, static_w=False)                               # P V
         x3 = torch.empty(S, C0, **act)
@@ -227,23 +188,14 @@ class _VAELowering:
             nm = f"up_blocks.{i}.upsamplers.0.conv"
             if (nm + ".w") in Wt:
                 up = torch.empty(4 * hh * ww, cout, **act)
-                P.upsample2x(x, B, hh, ww, cout, up, dtype=dt)
+                P.upsample_nearest(x, B, hh, ww, cout, up, 2 * hh, 2 * ww)
                 hh, ww = 2 * hh, 2 * ww
                 nx = torch.empty(hh * ww, cout, **act)
                 P.gemm(up, Wt[nm + ".w"], cout, B, hh, ww, nx, taps=9, bias=Wt[nm + ".b"])
                 x = nx
         no = sc("n1", hh * ww, cin)
-        P.groupnorm(x, B, hh * ww, cin, groups, Wt["norm_out.g"], Wt["norm_out.b"], 1e-6, 1, no, self.ws, dt)
+        P.groupnorm(x, B, hh * ww, cin, groups, Wt["norm_out.g"], Wt["norm_out.b"], 1e-6, 1, no, self.ws)
         img = torch.empty(1, 3, hh, ww, **act)
-        direct = os.environ.get("LB_CONV_OUT_DIRECT") is not None
-        if bf16 and direct:
-            raise _cabi.LB200Error("LB_CONV_OUT_DIRECT: the direct conv_out kernel is fp16-only; the bf16 VAE decoder "
-                                   "runs conv_out as an N = 8 GEMM (unset LB_CONV_OUT_DIRECT)")
-        if Wt.get("conv_out.w8") is not None and not direct:
-            # the direct 128 -> 3 kernel is far slower than the same convolution as an N = 8 GEMM
-            P.conv_out_gemm(no, B, hh, ww, cin, Wt["conv_out.w8"], Wt["conv_out.b8"], 3, img, sc("h1", hh * ww, 8), dt)
-        else:
-            P.conv_out(no, B, hh, ww, cin, Wt["conv_out.w"], Wt["conv_out.b"], 3, img)
-        P.postprocess_u8(img, self.frame, vae.nonfinite, dt)
-        self._keep = (scratch, z, hn, qk, vT, scores, x2, x3, x4, img)
+        lower_conv_out(P, Wt, no, B, hh, ww, cin, 3, img, sc)
+        P.postprocess_u8(img, self.frame, vae.nonfinite)
         P.finalize()

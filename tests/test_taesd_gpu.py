@@ -1,5 +1,5 @@
 """GPU tests of the tiny VAE decoder (AutoencoderTiny / TAESDXL): the depth-to-space GEMM (LB_GEMM_D2S2) against an
-fp32 upsample + conv, the tiny-VAE conv_in variant (lb_conv_in_act act 1), the whole decoder against the fp32 oracle
+fp32 upsample + conv, the tiny-VAE conv_in variant (lb_conv_in act 1), the whole decoder against the fp32 oracle
 (oracle/taesd.py) and its fixtures, and the engine running a transition with it.
 
 Tolerances (stated):
@@ -143,16 +143,16 @@ def test_conv_in_tiny_variant(h, w, in_scale):
     assert ops.error_flag() == 0
 
 
-def test_program_conv_in_act_plain_equals_conv_in():
-    """lb_conv_in_act with act 0 (through a program record) is lb_conv_in."""
-    from latentblending_b200 import ops
-    from latentblending_b200.unet import Program
+def test_program_conv_in_plain_record_equals_eager():
+    """A program conv_in record with act 0 (CONV_IN_PLAIN) is ops.conv_in's default."""
+    from latentblending_b200 import _cabi, ops
+    from latentblending_b200.program import Program
     lat = _rand(1, 4, 12, 20, seed=9).half()
     wt = (_rand(3, 3, 4, 64, seed=10) * 0.2).half()
     b = (_rand(64, seed=11) * 0.1).half()
     out = torch.empty(12 * 20, 64, dtype=torch.float16, device="cuda")
     P = Program(0)
-    P.conv_in_act(lat, wt, b, 64, out, 0)
+    P.conv_in(lat, wt, b, 64, out, _cabi.CONV_IN_PLAIN)
     P.finalize().run()
     assert torch.equal(out, ops.conv_in(lat, wt, b, 64))
 

@@ -258,7 +258,7 @@ def test_bf16_postprocess_counts_nonfinite():
 
 def test_program_rejects_bf16_on_fp16_only_kinds():
     from latentblending_b200 import _cabi
-    from latentblending_b200.unet import Program
+    from latentblending_b200.program import Program
     x = torch.zeros(64, 64, dtype=torch.float16, device="cuda")
     g = torch.ones(64, dtype=torch.float16, device="cuda")
     for build in (lambda P: P.layernorm(x, g, g, 1e-5, x),

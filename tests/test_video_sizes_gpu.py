@@ -50,26 +50,30 @@ def test_upsample_nearest_rejects_other_sizes():
         ops.upsample_nearest(_rand(30, 60)[:, :60], 2, 5, 3, 60, 10, 6)
 
 
-def test_upsample2x_and_program_default_unchanged():
-    """ops.upsample2x, ops.upsample_nearest at (2H, 2W) and a program op whose Ho, Wo are left at 0 give the same
-    bits."""
-    from latentblending_b200 import ops
-    from latentblending_b200.unet import Program
+def test_upsample2x_and_program_record_agree():
+    """ops.upsample2x, ops.upsample_nearest at (2H, 2W) and a program record give the same bits; a record's Ho, Wo
+    are explicit (0 is not a size)."""
+    from latentblending_b200 import _cabi, ops
+    from latentblending_b200.program import Program
     B, H, W, C = 2, 16, 24, 320
     x = _rand(B * H * W, C, seed=3)
     a = ops.upsample2x(x, B, H, W, C)
     b = ops.upsample_nearest(x, B, H, W, C, 2 * H, 2 * W)
     assert torch.equal(a, b)
     outs = []
-    for ho, wo in ((0, 0), (2 * H, 2 * W), (2 * H - 1, 2 * W - 1)):
-        out = torch.zeros(B * (ho or 2 * H) * (wo or 2 * W), C, dtype=torch.float16, device="cuda")
+    for ho, wo in ((2 * H, 2 * W), (2 * H - 1, 2 * W - 1)):
+        out = torch.zeros(B * ho * wo, C, dtype=torch.float16, device="cuda")
         P = Program(0)
-        P.upsample2x(x, B, H, W, C, out, ho, wo)
+        P.upsample_nearest(x, B, H, W, C, out, ho, wo)
         P.finalize().run()
         outs.append(out)
     torch.cuda.synchronize()
-    assert torch.equal(outs[0], a) and torch.equal(outs[1], a)
-    assert torch.equal(outs[2], ops.upsample_nearest(x, B, H, W, C, 2 * H - 1, 2 * W - 1))
+    assert torch.equal(outs[0], a)
+    assert torch.equal(outs[1], ops.upsample_nearest(x, B, H, W, C, 2 * H - 1, 2 * W - 1))
+    P = Program(0)
+    P.upsample_nearest(x, B, H, W, C, outs[0], 0, 0)
+    with pytest.raises(_cabi.LB200Error, match="nearest 2x"):
+        P.finalize().run()
     assert ops.error_flag() == 0
 
 
@@ -183,7 +187,7 @@ def test_full_sdxl_unet_runs_at_1080p():
 
 # ---- 3. VAE -------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("cols", [187, 5, 1, 192])
-def test_softmax_rows_any_width(cols):
+def test_softmax_rows_any_width_with_dtype(cols):
     """lb_softmax_rows over a column count that need not be a multiple of 8 (the VAE mid-block attention's h*w keys),
     in place in a wider buffer, vs torch.softmax in fp32; the columns past ``cols`` are left alone."""
     from latentblending_b200 import _cabi
@@ -192,7 +196,7 @@ def test_softmax_rows_any_width(cols):
     buf = _rand(rows, ld, seed=cols) * 4
     ref = torch.softmax(buf[:, :cols].float(), dim=-1)
     tail = buf[:, cols:].clone()
-    check(_cabi.load().lb_softmax_rows(ctx(0), ptr(buf), ld, rows, cols, ptr(buf), ld, stream_ptr()),
+    check(_cabi.load().lb_softmax_rows(ctx(0), ptr(buf), ld, rows, cols, ptr(buf), ld, stream_ptr(), _cabi.DTYPE_F16),
           "lb_softmax_rows")
     torch.cuda.synchronize()
     assert (buf[:, :cols].float() - ref).abs().max().item() <= 2e-3          # fp16 output rounding

@@ -1,4 +1,5 @@
-"""Micro-benchmarks of the UNet kernels at the SDXL 1024^2 shapes (CUDA-event timed)."""
+"""Micro-benchmarks of the UNet kernels at the SDXL 1024^2 shapes (CUDA-event timed).  Each op is recorded once into
+a one-record Program and replayed, as the lowered programs replay it."""
 import json
 import os
 import sys
@@ -6,7 +7,7 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from latentblending_b200 import ops  # noqa: E402
+from latentblending_b200.program import Program  # noqa: E402
 
 
 ITERS = int(os.environ.get('BENCH_ITERS', 20))
@@ -28,6 +29,13 @@ def time_it(fn, iters=None, warm=None):
     return s.elapsed_time(e) / iters * 1e-3
 
 
+def replay(emit):
+    """The run() of a one-record Program holding the op ``emit(P)`` records."""
+    P = Program(0)
+    emit(P)
+    return P.finalize().run
+
+
 def main():
     which = sys.argv[1:] or ["attn", "gemm"]
     if "attn" in which:
@@ -38,9 +46,9 @@ def main():
             kv = torch.randn(B * 77, 2 * C, device="cuda").half()
             out = torch.empty(B * S, C, device="cuda", dtype=torch.float16)
             if Skv == S:
-                f = lambda: ops.attention(qkv, qkv, qkv, out, B, heads, S, S, 0, C, 2 * C)
+                f = replay(lambda P: P.attention(qkv, qkv, qkv, out, B, heads, S, S, 0, C, 2 * C))
             else:
-                f = lambda: ops.attention(qkv, kv, kv, out, B, heads, S, 77, 0, 0, C)
+                f = replay(lambda P: P.attention(qkv, kv, kv, out, B, heads, S, 77, 0, 0, C))
             t = time_it(f)
             fl = 4 * B * heads * S * Skv * 64
             print(json.dumps(dict(op="attention", B=B, heads=heads, S=S, Skv=Skv, us=t * 1e6, tflops=fl / t / 1e12)))
@@ -55,14 +63,14 @@ def main():
                 a = torch.randn(M, K, device="cuda").half()
                 w = (torch.randn(N, 9 * K, device="cuda") * 0.02).half()
                 out = torch.empty(M, N, device="cuda", dtype=torch.float16)
-                f = lambda: ops.gemm(a, w, N, 2, hw, hw, taps=9, out=out)
+                f = replay(lambda P: P.gemm(a, w, N, 2, hw, hw, out, taps=9, static_w=False))
                 fl = 2 * M * N * 9 * K
             else:
                 a = torch.randn(M, K, device="cuda").half()
                 w = (torch.randn(N, K, device="cuda") * 0.02).half()
                 mode = 1 if "geglu" in name else 0
                 out = torch.empty(M, N // 2 if mode else N, device="cuda", dtype=torch.float16)
-                f = lambda: ops.gemm(a, w, N, 1, 1, M, out=out, mode=mode, static_w=True)
+                f = replay(lambda P: P.gemm(a, w, N, 1, 1, M, out, mode=mode))
                 fl = 2 * M * N * K
             t = time_it(f)
             print(json.dumps(dict(op="gemm", name=name, M=M, N=N, K=K * taps, us=round(t * 1e6, 1),
@@ -78,7 +86,7 @@ def vae_shapes():
         a = torch.randn(M, cin, device="cuda").half()
         w = (torch.randn(cout, 9 * cin, device="cuda") * 0.02).half()
         out = torch.empty(M, cout, device="cuda", dtype=torch.float16)
-        t = time_it(lambda: ops.gemm(a, w, cout, 1, hw, hw, taps=9, out=out, static_w=True), iters=5, warm=2)
+        t = time_it(replay(lambda P: P.gemm(a, w, cout, 1, hw, hw, out, taps=9)), iters=5, warm=2)
         fl = 2 * M * cout * 9 * cin
         print(json.dumps(dict(op="conv3x3", name=name, M=M, N=cout, K=9 * cin, us=round(t * 1e6, 1),
                               tflops=round(fl / t / 1e12, 1), cluster=os.environ.get("LB_GEMM_CLUSTER", "auto"))))

@@ -85,7 +85,7 @@ def decode_table(args, dev):
 def level_table(args, dev):
     from latentblending_b200 import ops
     from latentblending_b200.taesd import pack_d2s_weights
-    from latentblending_b200.unet import Program
+    from latentblending_b200.program import Program
     C = 64
     g = torch.Generator(device=dev).manual_seed(0)
     w = (torch.randn(C, C, 3, 3, generator=g, device=dev) * (9 * C) ** -0.5).half()
@@ -103,7 +103,7 @@ def level_table(args, dev):
         pd, pu = Program(0), Program(0)
         for _ in range(args.iters):
             pd.gemm(x, wd, 4 * C, 1, hh, hh, o1, taps=9, depth_to_space=True)
-            pu.upsample2x(x, 1, hh, hh, C, up)
+            pu.upsample_nearest(x, 1, hh, hh, C, up, 2 * hh, 2 * hh)
             pu.gemm(up, w3, C, 1, 2 * hh, 2 * hh, o2, taps=9)
         pd.finalize()
         pu.finalize()

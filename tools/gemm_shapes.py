@@ -12,6 +12,7 @@ batch 1; the default is config 2's lockstep-speculation split, cross-check it wi
 ``--root`` imports latentblending_b200 from another checkout (e.g. a build of an earlier commit) to compare builds.
 ``--latent HxW`` times the shapes of another output size (latent height x width, e.g. 152x104 for 832x1216 images);
 ``--tiling`` forces the GEMM's M tiling (the default lets lb_gemm choose; builds without the option need the default).
+Each shape is recorded once into a one-record Program and replayed, as the lowered programs replay it.
 The first line records the card, its power limit and its SM clocks (nvidia-smi, read-only).
 """
 import argparse
@@ -113,6 +114,10 @@ def main():
     import torch.nn.functional as F
     from latentblending_b200 import ops
     from latentblending_b200._cabi import LB200Error
+    try:
+        from latentblending_b200.program import Program
+    except ImportError:             # checkouts from before program.py
+        from latentblending_b200.unet import Program
     assert torch.cuda.is_available(), "gemm_shapes.py needs a CUDA device"
 
     sink = open(args.out, "a") if args.out else None
@@ -122,6 +127,12 @@ def main():
         print(line, flush=True)
         if sink:
             sink.write(line + "\n")
+
+    def gemm_run(*args, **kw):
+        """The run() of a one-record Program holding this GEMM."""
+        P = Program(0)
+        P.gemm(*args, **kw)
+        return P.finalize().run
 
     def time_it(fn, iters):
         for _ in range(3):
@@ -157,9 +168,8 @@ def main():
             out = torch.empty(M, N // 2 if geglu else N, device="cuda", dtype=torch.float16)
             wt = rnd(N, Ktot, s=Ktot ** -0.5)
             try:
-                us = time_it(lambda: ops.gemm(a, wt, N, B, h, w, taps=taps, a1=a1, bias=bias, res=r, out=out,
-                                              mode=(1 | args.geglu_flags) if geglu else 0, static_w=True, **tile_kw),
-                             args.iters)
+                us = time_it(gemm_run(a, wt, N, B, h, w, out, taps=taps, a1=a1, bias=bias, res=r,
+                                      mode=(1 | args.geglu_flags) if geglu else 0, **tile_kw), args.iters)
             except LB200Error as e:      # a build or tiling that cannot run this shape
                 emit(dict(op="unet_gemm", name=name, B=B, hw=h if h == w else f"{h}x{w}", error=str(e)))
                 continue
@@ -187,7 +197,7 @@ def main():
             wt = rnd(cout, 9 * cin, s=(9 * cin) ** -0.5)
             out = torch.empty(M, cout, device="cuda", dtype=torch.float16)
             try:
-                us = time_it(lambda: ops.gemm(a, wt, cout, 1, h, w, taps=9, out=out, static_w=True, **tile_kw), 5)
+                us = time_it(gemm_run(a, wt, cout, 1, h, w, out, taps=9, **tile_kw), 5)
             except LB200Error as e:
                 emit(dict(op="vae_conv3x3", name=name, h=h, w=w, error=str(e)))
                 continue
