@@ -8,6 +8,8 @@
 // diffusers 0.25.0 embeddings.py / resnet.py / unet_2d_condition.py).
 #include "common.cuh"
 
+#include <type_traits>
+
 namespace {
 
 constexpr int kThreads = 256;
@@ -543,7 +545,11 @@ nhwc_to_nchw_kernel(const __half* __restrict__ x, long long ld, int B, int C, lo
     }
 }
 
-// VaeImageProcessor.postprocess: NCHW fp16 image -> uint8 NHWC, (x/2+0.5).clamp(0,1)*255 rounded half-to-even.
+// VaeImageProcessor.postprocess: NCHW image -> uint8 NHWC, (x/2+0.5).clamp(0,1)*255 rounded half-to-even.
+// Each instantiation follows the reference chain of its decoder.  fp16 (an fp16-safe VAE, or the tiny VAE): the
+// reference decodes in fp16 and runs denormalize on that fp16 tensor, so x/2 and x/2 + 0.5 are each rounded to fp16
+// before the clamp; * 255 and the rounding are fp32 (numpy).  bf16 (an upcast VAE): the reference decodes in fp32,
+// so the whole chain is fp32.
 // `nonfinite` (optional) counts NaN/Inf pixels: the decoder runs in fp16 where the reference upcasts the stock SDXL VAE
 // to fp32 ("overflows in float16", diffusers_holder.py:128); an overflow anywhere upstream reaches the image as Inf/NaN.
 template <typename T>
@@ -559,7 +565,9 @@ postprocess_u8_kernel(const T* __restrict__ img, int B, int C, long long hw, uin
         const long long p = (i / C) % hw, b = i / (C * hw);
         const float raw = LbType<T>::to_f(img[(b * C + c) * hw + p]);
         bad += !isfinite(raw);
-        float v = raw / 2.0f + 0.5f;
+        float v;
+        if constexpr (std::is_same<T, __half>::value) v = lb_round_h(lb_round_h(raw / 2.0f) + 0.5f);
+        else v = raw / 2.0f + 0.5f;
         v = fminf(fmaxf(v, 0.f), 1.f);
         out[i] = (uint8_t)__float2int_rn(v * 255.0f);
     }

@@ -6,8 +6,9 @@
 // twice (stats pass, apply pass -- the second read is an L2 hit for every SDXL
 // activation) and writes once; LayerNorm is single-read (row kept in registers).
 // Deterministic and batch-invariant: fixed-order reductions, no floating-point atomics (one integer
-// "last block" counter per batch element finalises the statistics).  fp32 statistics, fp64 final
-// combine; output rounded to fp16 after the affine and again after SiLU, like the
+// "last block" counter per batch element finalises the statistics).  GroupNorm statistics are fp32 sums of x - K_g
+// (K_g: a pilot value of the group, so E[x^2] - mean^2 does not cancel when the mean is large next to sigma), fp64
+// final combine; output rounded to fp16 after the affine and again after SiLU, like the
 // reference's two separate torch ops.  GroupNorm also exists in bf16 (the bf16 VAE decoder): same statistics and
 // summation order, bf16 loads and roundings.
 #include "common.cuh"
@@ -27,6 +28,10 @@ __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)
 
 // pass 1: per (batch, row-chunk) partial sums per group; the last chunk of a batch element to finish turns the
 // partials into (mean, rstd) per group -- fixed summation order, fp64 combine, no floating-point atomics.
+// The sums are shifted: S1 = sum (x - K_g), S2 = sum (x - K_g)^2 with K_g = x[b, row 0, first channel of group g], so
+// mean = K_g + S1/n and var = S2/n - (S1/n)^2 lose no precision to a mean that is large next to sigma (unshifted fp32
+// sums of x and x^2 put an error of order 2^-24 mean^2 into the variance).  The pilot is per image, so results stay
+// batch-invariant.
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 gn_partial_kernel(const T* __restrict__ x, long long ld, int C, int HW, int groups, int rows_per_chunk,
@@ -49,11 +54,13 @@ gn_partial_kernel(const T* __restrict__ x, long long ld, int C, int HW, int grou
         const int cv = cv0 + (VP <= kThreads ? (int)threadIdx.x % VP : (int)threadIdx.x);
         const int rl = VP <= kThreads ? (int)threadIdx.x / VP : 0;
         const bool active = cv < VP && rl < RL;
-        float s[8], q[8];
+        float s[8], q[8], k[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
+        for (int j = 0; j < 8; ++j) s[j] = q[j] = k[j] = 0.f;
         if (active) {
             const T* col = base + 8 * cv;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) k[j] = LbType<T>::to_f(base[(8 * cv + j) / cpg * cpg]);    // K_g of channel
 #pragma unroll 4
             for (int r = row0 + rl; r < row1; r += RL) {
                 const uint4 v = *reinterpret_cast<const uint4*>(col + (long long)r * ld);
@@ -61,10 +68,11 @@ gn_partial_kernel(const T* __restrict__ x, long long ld, int C, int HW, int grou
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const float2 f = LbType<T>::to_f2(h[j]);
-                    s[2 * j] += f.x;
-                    s[2 * j + 1] += f.y;
-                    q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-                    q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
+                    const float d0 = f.x - k[2 * j], d1 = f.y - k[2 * j + 1];
+                    s[2 * j] += d0;
+                    s[2 * j + 1] += d1;
+                    q[2 * j] = fmaf(d0, d0, q[2 * j]);
+                    q[2 * j + 1] = fmaf(d1, d1, q[2 * j + 1]);
                 }
             }
         }
@@ -130,9 +138,10 @@ gn_partial_kernel(const T* __restrict__ x, long long ld, int C, int HW, int grou
                 tq += f_sq[sl * groups + threadIdx.x];
             }
             const double n = (double)HW * cpg;
-            const double mean = ts / n;
-            double var = tq / n - mean * mean;
+            const double m1 = ts / n;                                            // mean of x - K_g
+            double var = tq / n - m1 * m1;
             if (var < 0.0) var = 0.0;
+            const double mean = (double)LbType<T>::to_f(base[threadIdx.x * cpg]) + m1;
             stats[(long long)b * groups + threadIdx.x] = make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
         }
         if (threadIdx.x == 0) counter[b] = 0;       // ready for the next launch that shares this workspace
