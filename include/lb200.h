@@ -42,7 +42,7 @@
 extern "C" {
 #endif
 
-#define LB_ABI_VERSION 3
+#define LB_ABI_VERSION 4
 
 /* element type of the ops that exist in both 16-bit formats (lb_op.dtype, the trailing ``dtype`` arguments) */
 enum { LB_DTYPE_F16 = 0, LB_DTYPE_BF16 = 1 };
@@ -150,13 +150,6 @@ int lb_cfg_dpm_step(lb_ctx* ctx, const void* latents_dev, const void* eps_dev, c
  * conv2).  Epilogue mode 0: + bias[n] + bias2[b][n] (time-embedding projection)
  * + res[row][n]; mode 1: GEGLU, N accumulators -> N/2 outputs (weight rows
  * interleaved per 128-column tile: 64 value rows then their 64 gate rows).
- * LayerNorm fold (ln_stats != NULL; replaces the 210 torch.nn.LayerNorm launches of the transformer blocks): a0 holds
- * the UN-normalised rows x[M, K]; with w' = w * gamma (per input column), ln_csum[n] = sum_k w'[n,k] and
- * ln_bias[n] = sum_k beta[k] w[n,k] + bias[n] prepared once on the host,
- *     LN(x) w^T + bias  ==  rstd_m * (x w'^T - mu_m * ln_csum) + ln_bias,
- * where (mu_m, rstd_m) come from ln_stats[m][0..ln_parts) = per-row partial (sum, sum of squares) that the GEMM which
- * PRODUCED x wrote through its stats_out (of its stored fp16 values; stats_parts = 4 * ceil(N / its N tile), reported
- * by lb_gemm_stats_parts).  Fixed summation order: results do not depend on the batch size.
  * Replaces the cuBLAS / cuDNN calls under pipe.unet(...)
  * (diffusers_holder.py:336-344).  Constraints: a0_c, a1_c multiples of 64;
  * N multiple of 8; 16-byte aligned bases; any B, H, W with B*H*W < 2^31.
@@ -179,10 +172,6 @@ typedef struct lb_gemm_desc {
     void* out; int64_t out_ld;
     int32_t mode;     /* low byte: 0 = linear epilogue, 1 = GEGLU; flags: LB_GEMM_STATIC_W, LB_GEMM_RELU,
                          LB_GEMM_TILE_BOX, LB_GEMM_TILE_RUNS, LB_GEMM_BF16, LB_GEMM_OUT_F16, LB_GEMM_D2S2 */
-    const void* ln_stats; int32_t ln_parts;      /* float2 [M][ln_parts] or NULL */
-    const void* ln_csum; const void* ln_bias;    /* float [N] each */
-    float ln_eps;
-    void* stats_out; int32_t stats_parts;        /* float2 [M][stats_parts] or NULL (linear epilogue only) */
 } lb_gemm_desc;
 /* mode flag: `w` is not written by the kernel that precedes this one on the stream (true for model weights, false
  * when an activation is passed as the B operand): its first tiles may be fetched before the previous kernel ends. */
@@ -194,8 +183,8 @@ typedef struct lb_gemm_desc {
 #define LB_GEMM_TILE_BOX 0x400
 #define LB_GEMM_TILE_RUNS 0x800
 /* mode flag: a0, a1, w, bias, bias2, res and out are bf16 instead of fp16 (fp32 accumulation as in fp16; the output
- * is rounded to bf16).  Linear epilogue only: GEGLU, the LayerNorm fold and stats_out are rejected.  The VAE decoder of
- * a checkpoint whose activations overflow fp16 runs on it. */
+ * is rounded to bf16).  Linear epilogue only: GEGLU is rejected.  The VAE decoder of a checkpoint whose activations
+ * overflow fp16 runs on it. */
 #define LB_GEMM_BF16 0x1000
 /* mode flag, only with LB_GEMM_BF16: bf16 operands, fp16 output (the VAE attention scores, whose fp16 rounding is 8x
  * finer than bf16's and whose magnitudes stay far inside fp16's range; lb_softmax_rows reads them as fp16) */
@@ -206,13 +195,10 @@ typedef struct lb_gemm_desc {
  * filter's taps summed onto the low-resolution pixel they read after upsampling; see latentblending_b200/taesd.py).
  * Accumulator column p * Co + c of low-resolution pixel (img, y, x) is stored at output pixel (img, 2y + a, 2x + b),
  * channel c, of the NHWC output [4*B*H*W rows, row stride out_ld]: the upsampled input is never materialised.
- * fp16, linear epilogue (+ bias[N], LB_GEMM_RELU); rejected with res, bias2, a1, the LayerNorm fold, stats_out,
- * GEGLU or LB_GEMM_BF16, with taps != 9 and with N % 32 != 0 (so Co % 8 == 0). */
+ * fp16, linear epilogue (+ bias[N], LB_GEMM_RELU); rejected with res, bias2, a1, GEGLU or LB_GEMM_BF16, with
+ * taps != 9 and with N % 32 != 0 (so Co % 8 == 0). */
 #define LB_GEMM_D2S2 0x4000
 int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream);
-/* number of per-row partials a GEMM with this desc writes through stats_out (4 per N tile: one per lane of the quad
- * that holds a row of the wgmma accumulator); < 0 on error */
-int lb_gemm_stats_parts(lb_ctx* ctx, const lb_gemm_desc* desc);
 
 /* ---- K8: fused attention, head_dim 64 ----------------------------------------
  * out[b, s, h*64+d] = softmax(Q K^T * scale) V per (batch, head); Q/K/V are
@@ -257,9 +243,8 @@ int lb_layernorm(lb_ctx* ctx, const void* x, int64_t ld, int64_t rows, int C,
  * lb_linear_small: out = act_out(act_in(x) W^T + bias) (+ addend) for M <= 16 rows
  *   (time_embedding, add_embedding, all resnet time_emb_proj in one launch);
  *   act: 0 none, 1 SiLU.
- * lb_conv_in / lb_conv_out: the 4->C0 and C0->4 3x3 convolutions at the NCHW
- *   latent boundary.  lb_conv_in's ``act`` chooses an input transform and an
- *   output activation:
+ * lb_conv_in: the 4->C0 3x3 convolution at the NCHW latent boundary.  ``act``
+ *   chooses an input transform and an output activation:
  *   act 0: none (in_scale unused); x, w_packed, bias and out of type ``dtype``;
  *   act 1: the tiny VAE decoder's input stage (AutoencoderTiny:
  *          decoder(latents / scaling_factor), whose first steps are
@@ -285,8 +270,6 @@ int lb_linear_small(lb_ctx* ctx, const void* x, int64_t ldx, int M, int K, const
                     void* out, int64_t ldo, int N, void* stream);
 int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
                const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream, int dtype);
-int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,
-                const void* bias, int Cout, void* out_nchw, void* stream);
 int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
                         int Ho, int Wo, void* stream, int dtype);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
@@ -314,8 +297,7 @@ int lb_postprocess_u8(lb_ctx* ctx, const void* img_nchw, int B, int C, int64_t h
                       int* nonfinite_count_dev, void* stream, int dtype);
 /* lb_nhwc_to_nchw: the first C (<= 8) columns of NHWC rows [B*hw, ld] -> NCHW [B, C, hw].  The C0 -> 4 (UNet eps) and
  * C0 -> 3 (VAE RGB) output convolutions run as lb_gemm with an 8-row zero-padded weight matrix (N = 8); this puts the
- * result back into the reference's [B,C,H,W] tensor layout.  (lb_conv_out is the direct kernel for widths that are not
- * multiples of 64.) */
+ * result back into the reference's [B,C,H,W] tensor layout. */
 int lb_nhwc_to_nchw(lb_ctx* ctx, const void* x, int64_t ld, int B, int C, int64_t hw, void* out_nchw, void* stream,
                     int dtype);
 
@@ -354,11 +336,11 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * LB_OP_EMBED_INPUTS).  Replaces the module walk of pipe.unet(...)
  * (diffusers_holder.py:336-344).
  * lb_op.dtype: the ``dtype`` argument of the record's call for the kinds whose entry point takes one (above); it must
- * be 0 for every other kind (a GEMM takes its types from its mode flags).  Kind 18 is retired.
+ * be 0 for every other kind (a GEMM takes its types from its mode flags).  Kinds 8 and 18 are retired.
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
-    LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_CONV_OUT = 8, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
+    LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
     LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17
 };
@@ -375,7 +357,7 @@ typedef struct lb_op {
                  void* temb_in; void* add_in; } embed;
         struct { const void* x; int64_t ldx; int32_t M, K; const void* w; int64_t ldw; const void* bias;
                  const void* addend; int64_t ldadd; int32_t act_in, act_out; void* out; int64_t ldo; int32_t N; } lin;
-        /* CONV_IN, CONV_OUT (act, in_scale: lb_conv_in's; unused by CONV_OUT) */
+        /* CONV_IN (act, in_scale: lb_conv_in's) */
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
                  int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale; } conv;
         /* UPSAMPLE_NEAREST: output Ho x Wo (see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */

@@ -27,10 +27,7 @@ class GemmDesc(ctypes.Structure):
                 ("bias2", c_void_p), ("bias2_ld", c_int64),
                 ("res", c_void_p), ("res_ld", c_int64),
                 ("out", c_void_p), ("out_ld", c_int64),
-                ("mode", ctypes.c_int32),
-                ("ln_stats", c_void_p), ("ln_parts", ctypes.c_int32),
-                ("ln_csum", c_void_p), ("ln_bias", c_void_p), ("ln_eps", c_float),
-                ("stats_out", c_void_p), ("stats_parts", ctypes.c_int32)]
+                ("mode", ctypes.c_int32)]
 
 
 class AttnDesc(ctypes.Structure):
@@ -102,9 +99,10 @@ GEMM_BF16 = 0x1000        # LB_GEMM_BF16: bf16 operands, bias, residual and outp
 GEMM_OUT_F16 = 0x2000     # LB_GEMM_OUT_F16 (with GEMM_BF16): fp16 output
 GEMM_D2S2 = 0x4000        # LB_GEMM_D2S2: nearest-2x upsample + 3x3 conv as one GEMM, depth-to-space store
 DTYPE_F16, DTYPE_BF16 = 0, 1    # LB_DTYPE_F16 / LB_DTYPE_BF16: lb_op.dtype and the trailing dtype arguments
-(OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN, OP_CONV_OUT,
- OP_UPSAMPLE_NEAREST, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
- OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = range(1, 18)
+# lb_op.kind; kinds 8 and 18 are retired
+OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN = 1, 2, 3, 4, 5, 6, 7
+(OP_UPSAMPLE_NEAREST, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
+ OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = 9, 10, 11, 12, 13, 14, 15, 16, 17
 CONV_IN_PLAIN, CONV_IN_TINY_VAE = 0, 1     # lb_conv_in's act
 
 
@@ -129,7 +127,6 @@ SIGNATURES = {
                                 c_int64, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_float, c_float,
                                 c_void_p, c_int, c_float, c_void_p]),
     "lb_gemm": (c_int, [c_void_p, ctypes.POINTER(GemmDesc), c_void_p]),
-    "lb_gemm_stats_parts": (c_int, [c_void_p, ctypes.POINTER(GemmDesc)]),
     "lb_ctx_error_flag": (c_int, [c_void_p, ctypes.POINTER(c_int)]),
     "lb_program_create": (c_int, [c_void_p, ctypes.POINTER(Op), c_int64, ctypes.POINTER(c_void_p)]),
     "lb_program_run": (c_int, [c_void_p, c_float, c_void_p]),
@@ -150,8 +147,6 @@ SIGNATURES = {
                                 c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_void_p]),
     "lb_conv_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                            c_int64, c_int, c_float, c_void_p, c_int]),
-    "lb_conv_out": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
-                            c_void_p, c_void_p]),
     "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
                                     c_int, c_void_p, c_int]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -197,7 +192,7 @@ def load():
             fn = getattr(lib, name)       # AttributeError if the .so lacks a declared symbol
             fn.restype = res
             fn.argtypes = args
-        if lib.lb_abi_version() != 3:
+        if lib.lb_abi_version() != 4:
             raise LB200Error("liblb200.so ABI version mismatch")
         _lib = lib
     return _lib

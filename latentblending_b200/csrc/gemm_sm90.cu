@@ -28,8 +28,7 @@
 //                   registers, one k-block in flight while the previous one's slot is released.  A pair of
 //                   mbarriers lets one warpgroup at a time issue its main loop; the other meanwhile runs its epilogue
 //                   straight from the accumulators: + bias / per-batch bias (time embedding) / residual, or GEGLU,
-//                   or the LayerNorm fold, fp16 store.  So the tensor pipe keeps working through every epilogue
-//                   but a CTA's last.
+//                   fp16 store.  So the tensor pipe keeps working through every epilogue but a CTA's last.
 //                   BN = 256 (long-K convolutions only, see gemm_plan_build) does not fit one warpgroup's registers
 //                   at 128 rows: there both warpgroups work on every tile, 64 rows each (cooperative).
 // Weight (B operand) tiles of the first pipeline stages are requested BEFORE
@@ -57,7 +56,6 @@ namespace {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kEpiParts = 4;                 // stats_out partial sums per row and N tile: one per lane of a quad
 constexpr int kThreadsGemm = 384;            // warpgroup 0 TMA, warpgroups 1-2 wgmma + epilogue
 constexpr int kABytes = kBM * kBK * 2;  // 16 KiB
 constexpr int kGegluBN = 128;                // N tile of GEGLU launches (64 value + 64 gate columns)
@@ -90,37 +88,8 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return 0.5f * x * one_plus_erf;
 }
 
-__device__ __forceinline__ float2 ld_f2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 template <typename T> __device__ __forceinline__ typename LbType<T>::T2 ld_2(const T* p) {
     return __ldg(reinterpret_cast<const typename LbType<T>::T2*>(p));
-}
-
-// (mu, rstd) of one row of the LayerNorm-folded A operand from the producer's per-row partial sums (fixed order).
-// The partials of a row are contiguous (<= 64 x float2): they are fetched as float4 pairs, eight loads in flight at
-// a time.
-__device__ __forceinline__ void ln_row_stats(const GemmParams& p, long long row, bool ok, float& mu, float& rstd) {
-    mu = 0.f;
-    rstd = 1.f;
-    if (!ok) return;
-    float s = 0.f, q = 0.f;
-    const float4* st = reinterpret_cast<const float4*>(p.ln_stats + row * p.ln_parts);   // ln_parts is even
-    const int pairs = p.ln_parts >> 1;
-    for (int base = 0; base < pairs; base += 8) {
-        float4 v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = (base + i < pairs) ? __ldcg(st + base + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            s += v[i].x;
-            q += v[i].y;
-            s += v[i].z;
-            q += v[i].w;
-        }
-    }
-    mu = s * p.ln_inv_k;
-    double var = (double)q * (double)p.ln_inv_k - (double)mu * (double)mu;
-    if (var < 0.0) var = 0.0;
-    rstd = rsqrtf((float)var + p.ln_eps);
 }
 
 // One accumulator row of the current tile as the epilogue sees it.
@@ -128,15 +97,13 @@ struct EpiRow {
     long long row;     // output row (pixel index b*H*W + y*W + x)
     int bidx;          // batch index (bias2 row)
     bool ok;           // inside the output
-    float ln_mu, ln_rstd;
 };
 
 // Epilogues of one 64-row half of the tile.  The thread holds rows r[0], r[1] (acc[4j + 2i + e] is row r[i], column
 // 8j + 2*quad + e).  The global loads of a batch of column groups are all issued before any of its stores: the
 // residual may alias the output (in-place `hs += f(hs)`) and only this thread reads and writes these elements, so
 // the order is safe, and the loads overlap instead of costing one L2 round trip per 8-column group.
-// T: the element type of bias, bias2, res and out (bf16 kernels store fp16 instead when p.out_f16 is set); the
-// LayerNorm fold and stats_out exist in the fp16 kernels only.
+// T: the element type of bias, bias2, res and out (bf16 kernels store fp16 instead when p.out_f16 is set).
 // kD2S (LB_GEMM_D2S2, fp16 only): depth-to-space store.  Row r is low-resolution pixel (b, y, x) of a B x H x W map and
 // column n = ph * Co + c (Co = p.d2s_co, ph = 2a + b') goes to output pixel (b, 2y + a, 2x + b'), channel c, of the
 // B x 2H x 2W NHWC output.  Co % 8 == 0, so an 8-column group never straddles two phases; the phase of each group is
@@ -155,8 +122,7 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         if (!r[i].ok) continue;
-        float st_sum = 0.f, st_sq = 0.f;
-        // (no residual, bias2, LayerNorm fold or stats_out with depth-to-space: rejected on the host)
+        // (no residual or bias2 with depth-to-space: rejected on the host)
         const T* res_row = (!kD2S && p.res) ? reinterpret_cast<const T*>(p.res) + r[i].row * p.ldr : nullptr;
         const T* b2_row =
             (!kD2S && p.bias2) ? reinterpret_cast<const T*>(p.bias2) + (long long)r[i].bidx * p.bias2_ld : nullptr;
@@ -183,51 +149,32 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                 v[g][0] = acc[4 * (c0 + g) + 2 * i];
                 v[g][1] = acc[4 * (c0 + g) + 2 * i + 1];
             }
-            if (!kD2S && kF16 && p.ln_stats) {
-                constexpr int CL = CH > 8 ? CH / 2 : CH;     // fp32 vectors: half the batch
+            const T2 z = L::zero2();
+            T2 hb[CH], hb2[CH], hr[CH];
 #pragma unroll
-                for (int l0 = 0; l0 < CH; l0 += CL) {
-                    float2 c[CL], t[CL];
+            for (int g = 0; g < CH; ++g) {
+                const int n = n_base + 8 * (c0 + g);    // N is a multiple of 8 (checked on the host)
+                const bool in = n < p.N;
+                hb[g] = (p.bias && in) ? ld_2(reinterpret_cast<const T*>(p.bias) + n) : z;
+                hb2[g] = (b2_row && in) ? ld_2(b2_row + n) : z;
+                hr[g] = (res_row && in) ? *reinterpret_cast<const T2*>(res_row + n) : z;
+            }
 #pragma unroll
-                    for (int g = 0; g < CL; ++g) {
-                        const int n = n_base + 8 * (c0 + l0 + g);
-                        c[g] = n < p.N ? ld_f2(p.ln_csum + n) : make_float2(0.f, 0.f);
-                        t[g] = n < p.N ? ld_f2(p.ln_bias + n) : make_float2(0.f, 0.f);
-                    }
-#pragma unroll
-                    for (int g = 0; g < CL; ++g) {
-                        v[l0 + g][0] = fmaf(r[i].ln_rstd, v[l0 + g][0] - r[i].ln_mu * c[g].x, t[g].x);
-                        v[l0 + g][1] = fmaf(r[i].ln_rstd, v[l0 + g][1] - r[i].ln_mu * c[g].y, t[g].y);
-                    }
+            for (int g = 0; g < CH; ++g) {
+                if (p.bias) {
+                    const float2 t = L::to_f2(hb[g]);
+                    v[g][0] += t.x;
+                    v[g][1] += t.y;
                 }
-            } else {
-                const T2 z = L::zero2();
-                T2 hb[CH], hb2[CH], hr[CH];
-#pragma unroll
-                for (int g = 0; g < CH; ++g) {
-                    const int n = n_base + 8 * (c0 + g);    // N is a multiple of 8 (checked on the host)
-                    const bool in = n < p.N;
-                    hb[g] = (p.bias && in) ? ld_2(reinterpret_cast<const T*>(p.bias) + n) : z;
-                    hb2[g] = (b2_row && in) ? ld_2(b2_row + n) : z;
-                    hr[g] = (res_row && in) ? *reinterpret_cast<const T2*>(res_row + n) : z;
+                if (b2_row) {
+                    const float2 t = L::to_f2(hb2[g]);
+                    v[g][0] += t.x;
+                    v[g][1] += t.y;
                 }
-#pragma unroll
-                for (int g = 0; g < CH; ++g) {
-                    if (p.bias) {
-                        const float2 t = L::to_f2(hb[g]);
-                        v[g][0] += t.x;
-                        v[g][1] += t.y;
-                    }
-                    if (b2_row) {
-                        const float2 t = L::to_f2(hb2[g]);
-                        v[g][0] += t.x;
-                        v[g][1] += t.y;
-                    }
-                    if (res_row) {
-                        const float2 t = L::to_f2(hr[g]);
-                        v[g][0] += t.x;
-                        v[g][1] += t.y;
-                    }
+                if (res_row) {
+                    const float2 t = L::to_f2(hr[g]);
+                    v[g][0] += t.x;
+                    v[g][1] += t.y;
                 }
             }
 #pragma unroll
@@ -244,13 +191,7 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                         *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + orow * p.ldo + cc + 2 * quad) =
                             __floats2half2_rn(v0, v1);
                     } else if constexpr (kF16) {
-                        const __half2 o = __floats2half2_rn(v0, v1);
-                        *reinterpret_cast<__half2*>(out_row + n) = o;
-                        if (p.stats_out) {       // statistics of the STORED (fp16-rounded) values
-                            const float2 f = __half22float2(o);
-                            st_sum += f.x + f.y;
-                            st_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, st_sq));
-                        }
+                        *reinterpret_cast<__half2*>(out_row + n) = __floats2half2_rn(v0, v1);
                     } else if (p.out_f16) {      // the same 2-byte element address, fp16 value
                         *reinterpret_cast<__half2*>(out_row + n) = __floats2half2_rn(v0, v1);
                     } else {
@@ -263,8 +204,6 @@ __device__ __forceinline__ void epilogue_linear(const GemmParams& p, const float
                 }
             }
         }
-        if (!kD2S && kF16 && p.stats_out)
-            p.stats_out[r[i].row * (kEpiParts * p.tiles_n) + kEpiParts * n_tile + quad] = make_float2(st_sum, st_sq);
     }
 }
 
@@ -282,42 +221,19 @@ __device__ __forceinline__ void epilogue_geglu(const GemmParams& p, const float 
         if (!r[i].ok) continue;
         __half* out_row = p.out + r[i].row * p.ldo;
         float2 bv[G], bg[G];
-        if (p.ln_stats) {
-            float2 cv[G], cg[G];
 #pragma unroll
-            for (int j = 0; j < G; ++j) {
-                cv[j] = ld_f2(p.ln_csum + a_base + 8 * j);
-                cg[j] = ld_f2(p.ln_csum + a_base + HN + 8 * j);
-                bv[j] = ld_f2(p.ln_bias + a_base + 8 * j);
-                bg[j] = ld_f2(p.ln_bias + a_base + HN + 8 * j);
-            }
+        for (int j = 0; j < G; ++j) {
+            bv[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + 8 * j)) : make_float2(0.f, 0.f);
+            bg[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + HN + 8 * j)) : make_float2(0.f, 0.f);
+        }
+        // the reference rounds proj output, gelu(gate) and the product to fp16
 #pragma unroll
-            for (int j = 0; j < G; ++j) {
-                float v[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
-                float g[2] = {acc[4 * (j + G) + 2 * i], acc[4 * (j + G) + 2 * i + 1]};
-                v[0] = r[i].ln_rstd * (v[0] - r[i].ln_mu * cv[j].x);
-                v[1] = r[i].ln_rstd * (v[1] - r[i].ln_mu * cv[j].y);
-                g[0] = r[i].ln_rstd * (g[0] - r[i].ln_mu * cg[j].x);
-                g[1] = r[i].ln_rstd * (g[1] - r[i].ln_mu * cg[j].y);
-                // the reference rounds proj output, gelu(gate) and the product to fp16
-                const float r0 = lb_round_h(v[0] + bv[j].x) * lb_round_h(gelu_erf(lb_round_h(g[0] + bg[j].x)));
-                const float r1 = lb_round_h(v[1] + bv[j].y) * lb_round_h(gelu_erf(lb_round_h(g[1] + bg[j].y)));
-                *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < G; ++j) {
-                bv[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + 8 * j)) : make_float2(0.f, 0.f);
-                bg[j] = p.bias ? __half22float2(ld_2(p.bias + a_base + HN + 8 * j)) : make_float2(0.f, 0.f);
-            }
-#pragma unroll
-            for (int j = 0; j < G; ++j) {
-                const float r0 = lb_round_h(acc[4 * j + 2 * i] + bv[j].x) *
-                                 lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i] + bg[j].x)));
-                const float r1 = lb_round_h(acc[4 * j + 2 * i + 1] + bv[j].y) *
-                                 lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i + 1] + bg[j].y)));
-                *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
-            }
+        for (int j = 0; j < G; ++j) {
+            const float r0 = lb_round_h(acc[4 * j + 2 * i] + bv[j].x) *
+                             lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i] + bg[j].x)));
+            const float r1 = lb_round_h(acc[4 * j + 2 * i + 1] + bv[j].y) *
+                             lb_round_h(gelu_erf(lb_round_h(acc[4 * (j + G) + 2 * i + 1] + bg[j].y)));
+            *reinterpret_cast<__half2*>(out_row + o_base + 8 * j) = __floats2half2_rn(r0, r1);
         }
     }
 }
@@ -471,19 +387,6 @@ __device__ __forceinline__ void gemm_tc_body(const GemmParams& p) {
             e.row = ((long long)b * p.H + y) * p.W + x;
             e.bidx = b;
         };
-        // LayerNorm-fold row statistics: fetched before the main loop so their latency hides behind it
-        float ln_mu[kHalves][2], ln_rstd[kHalves][2];
-#pragma unroll
-        for (int hh = 0; hh < kHalves; ++hh)
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                ln_mu[hh][i] = 0.f;
-                ln_rstd[hh][i] = 1.f;
-                if (kF16 && p.ln_stats) {
-                    row_of(hh, i);
-                    ln_row_stats(p, er[hh][i].row, er[hh][i].ok, ln_mu[hh][i], ln_rstd[hh][i]);
-                }
-            }
         // this tile's k-blocks follow the j tiles before it in the ring
         const uint32_t it0 = (uint32_t)j * (uint32_t)p.total_kb;
         int stage = (int)(it0 % nst);
@@ -541,11 +444,7 @@ __device__ __forceinline__ void gemm_tc_body(const GemmParams& p) {
         // live range (the BN = 160 run kernel spills otherwise); the box kernels form all rows first.
         const auto rows_of_half = [&](int hh) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                row_of(hh, i);
-                er[hh][i].ln_mu = ln_mu[hh][i];
-                er[hh][i].ln_rstd = ln_rstd[hh][i];
-            }
+            for (int i = 0; i < 2; ++i) row_of(hh, i);
         };
         if constexpr (!kRuns) {
 #pragma unroll
@@ -740,15 +639,10 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
         LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_D2S2 supports the linear epilogue only (no GEGLU)");
         LB_REQUIRE(!bf16, "gemm: LB_GEMM_D2S2 is fp16-only (no LB_GEMM_BF16)");
         LB_REQUIRE(!d.res && !d.bias2 && !d.a1, "gemm: LB_GEMM_D2S2 takes no residual, bias2 or second input");
-        LB_REQUIRE(!d.ln_stats && !d.stats_out, "gemm: LB_GEMM_D2S2 does not support the LayerNorm fold or stats_out");
     }
     plan->d2s = d2s;
     LB_REQUIRE(bf16 || !(d.mode & LB_GEMM_OUT_F16), "gemm: LB_GEMM_OUT_F16 needs LB_GEMM_BF16");
-    if (bf16) {
-        LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_BF16 supports the linear epilogue only (no GEGLU)");
-        LB_REQUIRE(!d.ln_stats, "gemm: LB_GEMM_BF16 does not support the LayerNorm fold");
-        LB_REQUIRE(!d.stats_out, "gemm: LB_GEMM_BF16 does not support stats_out");
-    }
+    if (bf16) LB_REQUIRE((d.mode & 0xff) == 0, "gemm: LB_GEMM_BF16 supports the linear epilogue only (no GEGLU)");
     plan->bf16 = bf16;
     const int force = d.mode & (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS);
     LB_REQUIRE(force != (LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS), "gemm: LB_GEMM_TILE_BOX and LB_GEMM_TILE_RUNS exclude "
@@ -847,25 +741,6 @@ int gemm_plan_build(lb_ctx* ctx, const GemmDesc& d, GemmPlan* plan) {
     p.err_flag = lb_err_flag(ctx);
     p.relu = (d.mode & LB_GEMM_RELU) ? 1 : 0;
     LB_REQUIRE(!p.relu || p.mode == 0, "gemm: LB_GEMM_RELU needs the linear epilogue");
-    if (d.ln_stats) {
-        LB_REQUIRE(d.ln_csum && d.ln_bias && d.ln_parts >= 1 && d.ln_parts <= 64, "gemm: LayerNorm fold needs ln_csum, "
-                   "ln_bias and 1 <= ln_parts <= 64");
-        LB_REQUIRE(d.taps == 1 && !d.a1 && !d.res && !d.bias2 && !d.bias, "gemm: LayerNorm fold applies to a plain linear "
-                   "(its bias is part of ln_bias)");
-        LB_REQUIRE(lb_aligned16(d.ln_csum) && lb_aligned16(d.ln_bias) && lb_aligned16(d.ln_stats), "gemm: ln_* alignment");
-        p.ln_stats = static_cast<const float2*>(d.ln_stats);
-        p.ln_parts = d.ln_parts;
-        p.ln_csum = static_cast<const float*>(d.ln_csum);
-        p.ln_bias = static_cast<const float*>(d.ln_bias);
-        p.ln_inv_k = 1.0f / (float)d.a0_c;
-        p.ln_eps = d.ln_eps;
-    }
-    if (d.stats_out) {
-        LB_REQUIRE(p.mode == 0, "gemm: stats_out needs the linear epilogue");
-        LB_REQUIRE(d.stats_parts == kEpiParts * p.tiles_n, "gemm: stats_parts must be %d * ceil(N / %d) = %d (got %d)",
-                   kEpiParts, bn, kEpiParts * p.tiles_n, d.stats_parts);
-        p.stats_out = static_cast<float2*>(d.stats_out);
-    }
     {
         const int tiles = p.tiles_m * p.tiles_n;
         plan->grid = tiles < ctx->sm_count ? tiles : ctx->sm_count;
@@ -882,15 +757,6 @@ int gemm_plan_launch(const GemmPlan& plan, cudaStream_t st) {
     }
     lb_set_error("gemm: unsupported N tile %d", plan.bn);
     return 2;
-}
-
-extern "C" int lb_gemm_stats_parts(lb_ctx* ctx, const lb_gemm_desc* desc) {
-    if (!ctx || !desc) return -1;
-    GemmDesc d = *reinterpret_cast<const GemmDesc*>(desc);
-    d.stats_out = nullptr;
-    GemmPlan plan;
-    if (gemm_plan_build(ctx, d, &plan)) return -1;
-    return kEpiParts * plan.p.tiles_n;
 }
 
 extern "C" int lb_gemm(lb_ctx* ctx, const lb_gemm_desc* desc, void* stream) {

@@ -16,10 +16,6 @@ struct GemmDesc {
     void* out; int64_t out_ld;
     int32_t mode;   // low byte: 0 linear epilogue, 1 GEGLU (N accumulators -> N/2 outputs); | LB_GEMM_STATIC_W | LB_GEMM_RELU
                     // | LB_GEMM_TILE_BOX | LB_GEMM_TILE_RUNS | LB_GEMM_BF16 | LB_GEMM_OUT_F16 | LB_GEMM_D2S2
-    // LayerNorm folded into this GEMM (see include/lb200.h)
-    const void* ln_stats; int32_t ln_parts;
-    const void* ln_csum; const void* ln_bias; float ln_eps;
-    void* stats_out; int32_t stats_parts;
 };
 
 constexpr int kGemmMaxSegs = 12;
@@ -43,11 +39,6 @@ struct alignas(64) GemmParams {
     const __half* res; long long ldr;
     int* err_flag;
     int relu;      // mode 0: out = max(out, 0) (LB_GEMM_RELU)
-    // LayerNorm fold: A holds the UN-normalised rows x; out = rstd*(acc - mu*csum[n]) + lnb[n] with (mu, rstd) from the
-    // per-row partial sums the producing GEMM wrote (ln_stats[row][ln_parts] = (sum, sum of squares))
-    const float2* ln_stats; int ln_parts; float ln_inv_k, ln_eps;
-    const float* ln_csum; const float* ln_bias;
-    float2* stats_out;     // [M][4*tiles_n]: (sum, sum of squares) of this launch's fp16 outputs per row and column part
     // pixel-run tiling (runs = 1): tile m is rows [128 m, 128 m + 128) of the flattened b*H*W + y*W + x pixel order
     // (it may span image rows and images; M = B*H*W < 2^31), loaded by TMA im2col runs
     int runs;

@@ -2,7 +2,6 @@
 //   K3  timestep + added-condition embedding inputs (sinusoids) and the small-M linears
 //       (time_embedding, add_embedding, all resnet time_emb_proj in one batched launch)
 //   K2  conv_in  (4 -> C0, 3x3, NCHW latent in, NHWC out)
-//       conv_out (C0 -> 4, 3x3, NHWC in, NCHW eps out)
 //       nearest upsample (2x, or 2x cropped by one row / column), stride-2 im2col (the two Downsample2D convs then run as plain GEMMs)
 // Replace pieces of pipe.unet(...) (call site latentblending/diffusers_holder.py:336-344;
 // diffusers 0.25.0 embeddings.py / resnet.py / unet_2d_condition.py).
@@ -195,56 +194,6 @@ conv_in_tiny_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, 
     conv_in_body<__half, true>(x, B, Cin, H, W, wp, bias, Cout, out, ldo, in_scale);
 }
 
-// ---- conv_out: NHWC [B*H*W, Cin] -> NCHW [B,Cout<=4,H,W], 3x3 pad 1; one warp per pixel -----------
-// weights packed [co][ky][kx][Cin].
-__global__ void __launch_bounds__(kThreads)
-conv_out_kernel(const __half* __restrict__ x, long long ld, int B, int Cin, int H, int W,
-                const __half* __restrict__ wp, const __half* __restrict__ bias, int Cout, __half* __restrict__ out) {
-    pdl_launch_dependents();
-    pdl_wait();
-    extern __shared__ __half s_w[];   // [Cout][9][Cin]
-    const int wn = Cout * 9 * Cin;
-    for (int i = threadIdx.x; i < wn; i += kThreads) s_w[i] = wp[i];
-    __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long npix = (long long)B * H * W;
-    const int vecs = Cin >> 3;
-    for (long long pix = (long long)blockIdx.x * (kThreads / 32) + warp; pix < npix;
-         pix += (long long)gridDim.x * (kThreads / 32)) {
-        const int xw = (int)(pix % W), yh = (int)((pix / W) % H), b = (int)(pix / ((long long)W * H));
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int ky = 0; ky < 3; ++ky) {
-            const int yy = yh + ky - 1;
-            if (yy < 0 || yy >= H) continue;
-            for (int kx = 0; kx < 3; ++kx) {
-                const int xx = xw + kx - 1;
-                if (xx < 0 || xx >= W) continue;
-                const __half* src = x + (((long long)b * H + yy) * W + xx) * ld;
-                for (int v = lane; v < vecs; v += 32) {
-                    const uint4 xv = *reinterpret_cast<const uint4*>(src + v * 8);
-                    const __half2* xh = reinterpret_cast<const __half2*>(&xv);
-                    for (int co = 0; co < Cout; ++co) {
-                        const uint4 wv = *reinterpret_cast<const uint4*>(s_w + (co * 9 + ky * 3 + kx) * Cin + v * 8);
-                        const __half2* wh = reinterpret_cast<const __half2*>(&wv);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const float2 a = __half22float2(xh[j]);
-                            const float2 w2 = __half22float2(wh[j]);
-                            acc[co] = fmaf(a.x, w2.x, acc[co]);
-                            acc[co] = fmaf(a.y, w2.y, acc[co]);
-                        }
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int co = 0; co < 4; ++co) acc[co] = lb_warp_sum(acc[co]);
-        if (lane < Cout)
-            out[(((long long)b * Cout + lane) * H + yh) * W + xw] =
-                __float2half_rn(acc[lane] + __half2float(bias[lane]));
-    }
-}
-
 // ---- nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}), NHWC ------------------------------------
 // Nearest 2x cropped to Ho x Wo: output (yo, xo) reads input (yo >> 1, xo >> 1).  With H = ceil(Ho / 2) this is
 // exactly torch's nearest index min(floor(yo * (float)H / Ho), H - 1), so F.interpolate(size=...) needs no
@@ -383,27 +332,6 @@ extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H
                                                                             Cout, out, ldo, stream);
     return conv_in_launch<__half, conv_in_kernel<__half>>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo,
                                                           stream);
-}
-
-extern "C" int lb_conv_out(lb_ctx* ctx, const void* x, int64_t ld, int B, int Cin, int H, int W, const void* w_packed,
-                           const void* bias, int Cout, void* out_nchw, void* stream) {
-    LB_REQUIRE(ctx && x && w_packed && bias && out_nchw, "lb_conv_out: null argument");
-    LB_REQUIRE(Cout >= 1 && Cout <= 4 && Cin % 8 == 0 && ld % 8 == 0, "lb_conv_out: Cout<=4, Cin%%8==0 required");
-    const int smem = Cout * 9 * Cin * 2;
-    LB_REQUIRE(smem <= 96 * 1024, "lb_conv_out: weights do not fit shared memory");
-    static bool attr = false;
-    if (!attr) {
-        LB_CHECK_CUDA(cudaFuncSetAttribute(conv_out_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr = true;
-    }
-    const long long npix = (long long)B * H * W;
-    unsigned grid = (unsigned)lb_ceil_div(npix, kThreads / 32);
-    if (grid > (unsigned)ctx->sm_count * 8) grid = ctx->sm_count * 8;
-    lb_launch_pdl(conv_out_kernel, grid, kThreads, smem, lb_stream(stream), (const __half*)x, ld, B, Cin, H, W,
-                                                                (const __half*)w_packed, (const __half*)bias, Cout,
-                                                                (__half*)out_nchw);
-    LB_LAUNCH_CHECK();
-    return 0;
 }
 
 // the kernel moves 16-byte channel vectors, so fp16 and bf16 maps share it

@@ -92,7 +92,7 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_ATTENTION:
                 e = attn_plan_build_opaque(ctx, ops[i].u.attn, &nd.attn);
                 break;
-            case LB_OP_EMBED_INPUTS: case LB_OP_LINEAR_SMALL: case LB_OP_CONV_OUT:
+            case LB_OP_EMBED_INPUTS: case LB_OP_LINEAR_SMALL:
             case LB_OP_UPSAMPLE_NEAREST: case LB_OP_IM2COL_S2: case LB_OP_GROUPNORM: case LB_OP_LAYERNORM:
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
@@ -223,11 +223,6 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
                 const auto& a = o.u.conv;
                 e = lb_conv_in(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.act, a.in_scale,
                                stream, o.dtype);
-                break;
-            }
-            case LB_OP_CONV_OUT: {
-                const auto& a = o.u.conv;
-                e = lb_conv_out(ctx, a.x, a.ld_x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, stream);
                 break;
             }
             case LB_OP_UPSAMPLE_NEAREST: {

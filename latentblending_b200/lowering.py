@@ -1,11 +1,7 @@
 """Weight packing and lowering pieces the UNet (unet.py) and the KL VAE decoder (vae.py) share: the 3x3 conv
 weight layout, the resnet block (GroupNorm + SiLU, conv1, GroupNorm + SiLU, conv2 with the shortcut or the residual),
 the output convolution and the scratch buffers of a lowering."""
-import os
-
 import torch
-
-from . import _cabi
 
 
 def pack3(w):
@@ -69,15 +65,6 @@ def lower_resnet(P, W, r, x, cin, cout, B, h, w, out, groups, eps, ws, scratch, 
 
 
 def lower_conv_out(P, W, x, B, h, w, cin, cout, out_nchw, scratch):
-    """The 3x3 output convolution cin -> cout of ``x`` into NCHW ``out_nchw``: the N = 8 GEMM (``W['conv_out.w8']``,
-    present when cin is a multiple of 64; far faster than the direct kernel) then NCHW, or the direct fp16 kernel
-    when there is no w8 or LB_CONV_OUT_DIRECT is set.  The GEMM's [B*h*w, 8] output reuses the "h1" scratch."""
-    direct = os.environ.get("LB_CONV_OUT_DIRECT") is not None
-    if x.dtype == torch.bfloat16 and direct:
-        raise _cabi.LB200Error("LB_CONV_OUT_DIRECT: the direct conv_out kernel is fp16-only; the bf16 VAE decoder "
-                               "runs conv_out as an N = 8 GEMM (unset LB_CONV_OUT_DIRECT)")
-    if W.get("conv_out.w8") is not None and not direct:
-        P.conv_out_gemm(x, B, h, w, cin, W["conv_out.w8"], W["conv_out.b8"], cout, out_nchw,
-                        scratch("h1", B * h * w, 8))
-    else:
-        P.conv_out(x, B, h, w, cin, W["conv_out.w"], W["conv_out.b"], cout, out_nchw)
+    """The 3x3 output convolution cin -> cout of ``x`` into NCHW ``out_nchw``: the N = 8 GEMM
+    (``W['conv_out.w8']``, ``pack_conv_out8``) then NCHW.  The GEMM's [B*h*w, 8] output reuses the "h1" scratch."""
+    P.conv_out_gemm(x, B, h, w, cin, W["conv_out.w8"], W["conv_out.b8"], cout, out_nchw, scratch("h1", B * h * w, 8))

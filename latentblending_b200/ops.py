@@ -7,7 +7,7 @@ import torch
 
 from . import _cabi
 from ._cabi import check, ctx, ptr, stream_ptr
-from .program import LAUNCHES, Program
+from .program import LAUNCHES, Program, pack_conv_out8
 
 _DT = {torch.float16: 0, torch.float32: 1}
 
@@ -160,7 +160,7 @@ def _run1(dev, emit, t=0.0):
 
 
 def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None, out=None,
-         mode=0, out_cols=None, static_w=False, relu=False, ln=None, stats_out=None, tiling="auto", out_dtype=None,
+         mode=0, out_cols=None, static_w=False, relu=False, tiling="auto", out_dtype=None,
          depth_to_space=False):
     """Tensor-core GEMM / implicit-GEMM conv (``Program.gemm``).  The output (allocated unless ``out`` is given) is
     [B*H*W, N] (N/2 with GEGLU, ``out_cols`` when given), or [B*2H*2W, N/4] with ``depth_to_space``, of type
@@ -176,15 +176,9 @@ def gemm(a0, w, N, B, H, W, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bi
         shape = (4 * M, N // 4) if depth_to_space else (M, n_out)
         out = torch.empty(shape, dtype=out_dtype, device=a0.device)
     _run1(dev, lambda P: P.gemm(a0, w, N, B, H, W, out, taps=taps, a0_c=a0_c, a1=a1, a1_c=a1_c, bias=bias,
-                                bias2=bias2, res=res, mode=mode, static_w=static_w, relu=relu, ln=ln,
-                                stats_out=stats_out, tiling=tiling, depth_to_space=depth_to_space))
+                                bias2=bias2, res=res, mode=mode, static_w=static_w, relu=relu, tiling=tiling,
+                                depth_to_space=depth_to_space))
     return out
-
-
-def gemm_stats_parts(a0, w, N, B, H, W, **kw):
-    """Per-row partial count of lb_gemm's stats_out for this problem (4 per N tile)."""
-    out = torch.empty((B * H * W, N), dtype=torch.float16, device=a0.device)
-    return Program(_dev(a0)).gemm_stats_parts(a0, w, N, B, H, W, out, **kw)
 
 
 def lpips_tap(feat_a, feat_b, lin_w, out_scalar, workspace, accumulate=False):
@@ -274,10 +268,14 @@ def conv_in(x_nchw, w_packed, bias, Cout, out=None, act=_cabi.CONV_IN_PLAIN, in_
 
 
 def conv_out(x, B, H, W, Cin, w_packed, bias, Cout, out=None):
+    """The Cin -> Cout 3x3 output convolution of NHWC ``x`` into NCHW, as the lowerings run it: ``w_packed``
+    [Cout][3][3][Cin] through ``pack_conv_out8``, then ``Program.conv_out_gemm``."""
     dev = _dev(x)
+    w8, b8 = pack_conv_out8(w_packed, bias)
     if out is None:
-        out = torch.empty((B, Cout, H, W), dtype=torch.float16, device=x.device)
-    _run1(dev, lambda P: P.conv_out(x, B, H, W, Cin, w_packed, bias, Cout, out))
+        out = torch.empty((B, Cout, H, W), dtype=x.dtype, device=x.device)
+    tmp = torch.empty((B * H * W, 8), dtype=x.dtype, device=x.device)
+    _run1(dev, lambda P: P.conv_out_gemm(x, B, H, W, Cin, w8, b8, Cout, out, tmp))
     return out
 
 

@@ -7,7 +7,7 @@ import ctypes
 import torch
 
 from . import _cabi
-from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_CONV_OUT, OP_EMBED_INPUTS, OP_GEMM,
+from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_EMBED_INPUTS, OP_GEMM,
                     OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
                     OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS,
                     OP_UPSAMPLE_NEAREST, Op, check, ctx, stream_ptr)
@@ -68,7 +68,7 @@ class Program:
 
     # -- op emitters ---------------------------------------------------------------------------
     def gemm(self, a0, w, N, B, H, W, out, taps=1, a0_c=None, a1=None, a1_c=None, bias=None, bias2=None, res=None,
-             mode=0, static_w=True, relu=False, ln=None, stats_out=None, tiling="auto", depth_to_space=False):
+             mode=0, static_w=True, relu=False, tiling="auto", depth_to_space=False):
         """Tensor-core GEMM / implicit-GEMM conv (lb_gemm_desc).  a0: NHWC activation viewed as [B*H*W, >=a0_c]
         (row stride = a0.stride(-2)); w: [N, K] packed weights.
         ``static_w``: ``w`` holds model weights (not written by the preceding op), so the kernel may fetch its
@@ -78,9 +78,6 @@ class Program:
         same results.
         ``depth_to_space``: nearest-2x upsample + 3x3 conv as one GEMM (LB_GEMM_D2S2): ``w`` holds the four phase
         filters [4*Co, 9*C] (``taesd.pack_d2s_weights``), ``out`` the [B*2H*2W, Co] upsampled map.
-        ``ln``: dict(stats=[M,parts,2] fp32, csum=[N] fp32, bias=[N] fp32, eps) -- LayerNorm folded into this GEMM
-        (``w`` must already hold w*gamma; see include/lb200.h).  ``stats_out``: [M,parts,2] fp32 buffer that receives
-        this GEMM's per-row partial sums for a following LN-folded GEMM (parts = self.gemm_stats_parts(...)).
         Element types come from the tensors: fp16 throughout, or bf16 a0 / w / a1 / bias / bias2 / res
         (LB_GEMM_BF16) writing ``out``'s type (bf16, or fp16: LB_GEMM_OUT_F16)."""
         if tiling not in _TILING:
@@ -101,26 +98,7 @@ class Program:
         d.mode = mode | (GEMM_STATIC_W if static_w else 0) | (GEMM_RELU if relu else 0) | _TILING[tiling] | dmode
         if depth_to_space:
             d.mode |= _cabi.GEMM_D2S2
-        if ln is not None:
-            st = ln["stats"]
-            assert st.dtype == torch.float32 and st.dim() == 3 and st.shape[2] == 2 and st.is_contiguous()
-            d.ln_stats, d.ln_parts = _p(st), st.shape[1]
-            d.ln_csum, d.ln_bias, d.ln_eps = _p(ln["csum"]), _p(ln["bias"]), ln["eps"]
-            self.hold(st, ln["csum"], ln["bias"])
-        if stats_out is not None:
-            assert stats_out.dtype == torch.float32 and stats_out.dim() == 3 and stats_out.is_contiguous()
-            d.stats_out, d.stats_parts = _p(stats_out), stats_out.shape[1]
-            self.hold(stats_out)
         self.hold(a0, w, a1, bias, bias2, res, out)
-
-    def gemm_stats_parts(self, a0, w, N, B, H, W, out, **kw):
-        """Number of per-row partials a GEMM with these arguments writes through ``stats_out``."""
-        probe = Program(self.dev)
-        probe.gemm(a0, w, N, B, H, W, out, **kw)
-        n = int(_cabi.load().lb_gemm_stats_parts(ctx(self.dev), ctypes.byref(probe.ops[0].u.gemm)))
-        if n < 0:
-            raise _cabi.LB200Error("lb_gemm_stats_parts failed: " + _cabi.load().lb_last_error().decode())
-        return n
 
     def lpips_im2col_u8(self, frame_u8, H, W, k, stride, pad, shift, scale, out):
         d = self._new(OP_LPIPS_IM2COL_U8).u.patch
@@ -193,13 +171,6 @@ class Program:
         d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
         d.out, d.ld_out, d.act, d.in_scale = _p(out), out.stride(0), int(act), float(in_scale)
         self.hold(x_nchw, w, bias, out)
-
-    def conv_out(self, x, B, H, W, Cin, w, bias, Cout, out_nchw):
-        """The direct fp16 C0 -> Cout (<= 4) kernel (lb_conv_out)."""
-        d = self._new(OP_CONV_OUT).u.conv
-        d.x, d.ld_x, d.B, d.Cin, d.H, d.W = _p(x), x.stride(0), B, Cin, H, W
-        d.w, d.bias, d.Cout, d.out = _p(w), _p(bias), Cout, _p(out_nchw)
-        self.hold(x, w, bias, out_nchw)
 
     def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp):
         """The C0 -> Cout (<= 8) 3x3 output convolution on the tensor-core GEMM: N = 8 (zero-padded weight rows),
@@ -306,11 +277,12 @@ class Program:
 
 
 def pack_conv_out8(w_co_ky_kx_ci, bias):
-    """[Cout<=8][3][3][Cin] conv_out weights -> ([8, 9*Cin] zero-padded rows, [8] bias) for the N = 8 GEMM; None when
-    Cin is not a multiple of 64 (the GEMM's K blocks) -- the direct lb_conv_out kernel is used then."""
+    """[Cout<=8][3][3][Cin] conv_out weights -> ([8, 9*Cin] zero-padded rows, [8] bias) for the N = 8 GEMM.  Raises
+    LB200Error when Cin is not a multiple of 64 (the GEMM's K blocks) or Cout > 8."""
     co, cin = w_co_ky_kx_ci.shape[0], w_co_ky_kx_ci.shape[-1]
     if cin % 64 != 0 or co > 8:
-        return None, None
+        raise _cabi.LB200Error(f"conv_out: the N = 8 GEMM needs Cin % 64 == 0 and Cout <= 8 (got Cin {cin}, "
+                               f"Cout {co})")
     w8 = torch.zeros(8, 9 * cin, dtype=w_co_ky_kx_ci.dtype, device=w_co_ky_kx_ci.device)     # fp16, or bf16
     w8[:co] = w_co_ky_kx_ci.reshape(co, 9 * cin)
     b8 = torch.zeros(8, dtype=bias.dtype, device=bias.device)

@@ -54,16 +54,6 @@ class UNetConfig:
         return self.pooled_dim + 6 * self.addition_time_embed_dim
 
 
-def _fold_layernorm(w, bias, gamma, beta):
-    """(w*gamma in fp16, rowsum of THAT in fp32, w beta + bias in fp32) for the LayerNorm-folded GEMM."""
-    wf = (w.float() * gamma.float()[None, :]).half().contiguous()
-    csum = wf.float().sum(dim=1).contiguous()
-    lnb = w.float() @ beta.float()
-    if bias is not None:
-        lnb = lnb + bias.float()
-    return wf, csum, lnb.contiguous()
-
-
 def guidance_scale_embedding(guidance_scale, dim):
     """[1, dim] fp16 CPU guidance-scale embedding of a time-conditioned UNet (LCM-SDXL's ``timestep_cond``), computed
     as the reference does (diffusers_holder.py:304-309 via the pipeline's get_guidance_scale_embedding):
@@ -89,10 +79,9 @@ def _geglu_perm(inner, device, half=64):
 class PackedUNet:
     """fp16 device copies of the UNet parameters in the layouts the kernels consume."""
 
-    def __init__(self, cfg: UNetConfig, state_dict, device, fold_ln=True):
+    def __init__(self, cfg: UNetConfig, state_dict, device):
         self.cfg = cfg
         self.device = torch.device(device)
-        self.fold_ln = fold_ln
         sd = state_dict
         dev = self.device
 
@@ -104,9 +93,8 @@ class PackedUNet:
         W = self.w
         W["conv_in.w"] = g("conv_in.weight").permute(2, 3, 1, 0).contiguous()      # [ky][kx][cin][Cout]
         W["conv_in.b"] = g("conv_in.bias")
-        W["conv_out.w"] = g("conv_out.weight").permute(0, 2, 3, 1).contiguous()     # [co][ky][kx][Cin]
-        W["conv_out.b"] = g("conv_out.bias")
-        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(W["conv_out.w"], W["conv_out.b"])
+        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(g("conv_out.weight").permute(0, 2, 3, 1),
+                                                            g("conv_out.bias"))
         for nm in ("conv_norm_out",):
             W[nm + ".g"], W[nm + ".b"] = g(nm + ".weight"), g(nm + ".bias")
         for e in ("time_embedding", "add_embedding"):
@@ -155,18 +143,8 @@ class PackedUNet:
                 W[t + ".attn2.out.w"], W[t + ".attn2.out.b"] = g(t + ".attn2.to_out.0.weight"), g(t + ".attn2.to_out.0.bias")
                 pw, pb = g(t + ".ff.net.0.proj.weight"), g(t + ".ff.net.0.proj.bias")
                 perm = _geglu_perm(pw.shape[0] // 2, dev)     # per 128-column N tile of the GEGLU GEMM
-                if fold_ln:
-                    # LayerNorm folded into the consuming GEMM (include/lb200.h): w' = w*gamma, csum = rowsum(w'),
-                    # lnb = w beta + bias
-                    for key, w_, b_, nrm, pm in ((".attn1.qkv", wqkv, None, "norm1", None), (".attn2.q", wq, None, "norm2", None),
-                                                 (".ff.in", pw, pb, "norm3", perm)):
-                        wf, cs, lb = _fold_layernorm(w_, b_, W[f"{t}.{nrm}.g"], W[f"{t}.{nrm}.b"])
-                        if pm is not None:
-                            wf, cs, lb = wf[pm].contiguous(), cs[pm].contiguous(), lb[pm].contiguous()
-                        W[t + key + ".w"], W[t + key + ".csum"], W[t + key + ".lnb"] = wf, cs, lb
-                else:
-                    W[t + ".attn1.qkv.w"], W[t + ".attn2.q.w"] = wqkv, wq
-                    W[t + ".ff.in.w"], W[t + ".ff.in.b"] = pw[perm].contiguous(), pb[perm].contiguous()
+                W[t + ".attn1.qkv.w"], W[t + ".attn2.q.w"] = wqkv, wq
+                W[t + ".ff.in.w"], W[t + ".ff.in.b"] = pw[perm].contiguous(), pb[perm].contiguous()
                 W[t + ".ff.out.w"], W[t + ".ff.out.b"] = g(t + ".ff.net.2.weight"), g(t + ".ff.net.2.bias")
                 depth += 1
             W[a + ".depth"] = depth
@@ -182,18 +160,11 @@ class PackedUNet:
 class UNetB200:
     """One lowered forward per (batch, h, w); ``forward`` replays it."""
 
-    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0", fold_ln=None):
-        import os
+    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0"):
         self.cfg = cfg
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
-        # LayerNorm folding is OFF by default: the 210 LayerNorm launches need no shared memory, so under PDL they
-        # co-reside with the neighbouring GEMMs' CTAs; folding them away makes GEMM follow GEMM and adds epilogue work.
-        # LB_LN_FOLD=1 or fold_ln=True enables the folded path (same numerics and tolerance).
-        if fold_ln is None:
-            fold_ln = os.environ.get("LB_LN_FOLD") is not None
-        self.fold_ln = fold_ln
-        self.packed = PackedUNet(cfg, state_dict, self.device, fold_ln=fold_ln)
+        self.packed = PackedUNet(cfg, state_dict, self.device)
         self._plans = {}
 
     # -- public -----------------------------------------------------------------------------
@@ -253,7 +224,6 @@ class _Lowering:
         P = self.prog_step = Program(net.dev_index)
         PC = self.prog_ctx = Program(net.dev_index)
         scratch = Scratch(torch.float16, dev)
-        ln_stats = {}
 
         self._persist = []
 
@@ -318,9 +288,7 @@ class _Lowering:
 
         kv_cache = {}
 
-        fold = net.fold_ln
         geglu_mode = 1
-        f32 = dict(dtype=torch.float32, device=dev)
 
         def transformer(aname, x, C, level, out):
             h_, w_ = res_hw[level]
@@ -330,21 +298,7 @@ class _Lowering:
             tn = scratch("tn", M, C)
             P.groupnorm(x, B, S, C, groups, Wt[aname + ".norm.g"], Wt[aname + ".norm.b"], 1e-6, 0, tn, self.ws)
             hs = scratch("hs", M, C)
-            if not fold:
-                P.gemm(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs, bias=Wt[aname + ".proj_in.b"])
-                stats = None
-            else:
-                # every GEMM that writes the residual stream ``hs`` also writes its per-row partial sums; the three
-                # LayerNorms of a block are folded into the GEMMs that consume them (no LN launches, no LN buffer)
-                parts = P.gemm_stats_parts(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs)
-                if (M, parts) not in ln_stats:
-                    ln_stats[(M, parts)] = torch.zeros(M, parts, 2, **f32)
-                stats = ln_stats[(M, parts)]
-                P.gemm(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs, bias=Wt[aname + ".proj_in.b"], stats_out=stats)
-
-            def ln_of(t, key):
-                return dict(stats=stats, csum=Wt[t + key + ".csum"], bias=Wt[t + key + ".lnb"], eps=1e-5)
-
+            P.gemm(tn, Wt[aname + ".proj_in.w"], C, 1, 1, M, hs, bias=Wt[aname + ".proj_in.b"])
             for d in range(Wt[aname + ".depth"]):
                 t = f"{aname}.transformer_blocks.{d}"
                 qkv = scratch("qkv", M, 3 * C)
@@ -354,16 +308,6 @@ class _Lowering:
                 kv = persist(B * 77, 2 * C)         # depends on the conditioning only: computed by prog_ctx
                 PC.gemm(self.ctx, Wt[t + ".attn2.kv.w"], 2 * C, 1, 1, B * 77, kv)
                 kv_cache[t] = kv
-                if fold:
-                    P.gemm(hs, Wt[t + ".attn1.qkv.w"], 3 * C, 1, 1, M, qkv, ln=ln_of(t, ".attn1.qkv"))
-                    P.attention(qkv, qkv, qkv, att, B, heads, S, S, 0, C, 2 * C, cfg.head_dim ** -0.5)
-                    P.gemm(att, Wt[t + ".attn1.out.w"], C, 1, 1, M, hs, bias=Wt[t + ".attn1.out.b"], res=hs, stats_out=stats)
-                    P.gemm(hs, Wt[t + ".attn2.q.w"], C, 1, 1, M, q, ln=ln_of(t, ".attn2.q"))
-                    P.attention(q, kv, kv, att, B, heads, S, 77, 0, 0, C, cfg.head_dim ** -0.5)
-                    P.gemm(att, Wt[t + ".attn2.out.w"], C, 1, 1, M, hs, bias=Wt[t + ".attn2.out.b"], res=hs, stats_out=stats)
-                    P.gemm(hs, Wt[t + ".ff.in.w"], 8 * C, 1, 1, M, gg, mode=geglu_mode, ln=ln_of(t, ".ff.in"))
-                    P.gemm(gg, Wt[t + ".ff.out.w"], C, 1, 1, M, hs, bias=Wt[t + ".ff.out.b"], res=hs, stats_out=stats)
-                    continue
                 ln = scratch("ln", M, C)
                 P.layernorm(hs, Wt[t + ".norm1.g"], Wt[t + ".norm1.b"], 1e-5, ln)
                 P.gemm(ln, Wt[t + ".attn1.qkv.w"], 3 * C, 1, 1, M, qkv)

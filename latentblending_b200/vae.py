@@ -108,12 +108,8 @@ class VAEDecoderB200(DecoderBase):
                 nm = k[: -len(".weight")]
                 W[nm + ".w"], W[nm + ".b"] = pack3(g(nm + ".weight")), g(nm + ".bias")
         W["norm_out.g"], W["norm_out.b"] = g("conv_norm_out.weight"), g("conv_norm_out.bias")
-        W["conv_out.w"] = g("conv_out.weight").permute(0, 2, 3, 1).contiguous()
-        W["conv_out.b"] = g("conv_out.bias")
-        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(W["conv_out.w"], W["conv_out.b"])
-        if dtype == torch.bfloat16 and W["conv_out.w8"] is None:
-            raise _cabi.LB200Error("the bf16 VAE decoder runs conv_out as an N = 8 GEMM, which needs a multiple of 64 "
-                                   f"channels there (got {W['conv_out.w'].shape[-1]})")
+        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(g("conv_out.weight").permute(0, 2, 3, 1),
+                                                            g("conv_out.bias"))
     def _lower(self, h, w):
         return _VAELowering(self, h, w)
 

@@ -203,12 +203,11 @@ def test_engine_refuses_random_lpips_for_real_weights():
         BlendingEngine(RealPipe(), holder=dh, run_benchmark=False)
 
 
-def test_layernorm_fold_algebra_and_geglu_permutation_on_cpu():
-    """Host-side packing of the optional LayerNorm fold (unet._fold_layernorm) and of the GEGLU row interleave
-    (unet._geglu_perm), checked in fp32 on the CPU against torch's LayerNorm + Linear + exact-erf GEGLU: the kernel
-    computes rstd*(x W'^T - mu*csum) + lnb per row, and reads value / gate rows per N tile."""
+def test_geglu_permutation_on_cpu():
+    """Host-side GEGLU row interleave (unet._geglu_perm), checked in fp32 on the CPU against torch's LayerNorm +
+    Linear + exact-erf GEGLU: the kernel reads value / gate rows per N tile."""
     import torch.nn.functional as F
-    from latentblending_b200.unet import _fold_layernorm, _geglu_perm
+    from latentblending_b200.unet import _geglu_perm
     g = torch.Generator().manual_seed(0)
     M, C, N = 37, 128, 512
     x = torch.randn(M, C, generator=g) * 2 + 0.5
@@ -216,14 +215,7 @@ def test_layernorm_fold_algebra_and_geglu_permutation_on_cpu():
     b = (torch.randn(N, generator=g) * 0.1).half()
     gamma = (1 + 0.1 * torch.randn(C, generator=g)).half()
     beta = (0.05 * torch.randn(C, generator=g)).half()
-    wf, csum, lnb = _fold_layernorm(w, b, gamma, beta)
-    assert wf.dtype == torch.float16 and csum.dtype == lnb.dtype == torch.float32
-    mu = x.mean(1, keepdim=True)
-    rstd = (x.var(1, unbiased=False, keepdim=True) + 1e-5).rsqrt()
-    got = rstd * (x @ wf.float().t() - mu * csum[None, :]) + lnb[None, :]
     want = F.layer_norm(x, (C,), gamma.float(), beta.float(), 1e-5) @ w.float().t() + b.float()
-    # the only difference is the fp16 rounding of w*gamma
-    assert ((got - want).norm() / want.norm()).item() < 1e-3
     # GEGLU interleave: tile t of `half` value rows is followed by its `half` gate rows
     for half in (64, 128):
         perm = _geglu_perm(N // 2, "cpu", half=half)

@@ -29,11 +29,11 @@ def test_header_symbols_exported(lib_path):
         assert hasattr(lib, n), f"{n} declared in include/lb200.h but not exported"
 
 
-def test_ctypes_signatures_cover_header_abi3(lib_path):
+def test_ctypes_signatures_cover_header_abi4(lib_path):
     from latentblending_b200 import _cabi
     assert sorted(_cabi.SIGNATURES) == _declared()
     lib = _cabi.load()
-    assert lib.lb_abi_version() == 3
+    assert lib.lb_abi_version() == 4
 
 
 def test_product_never_imports_oracle():

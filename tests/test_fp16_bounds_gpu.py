@@ -311,36 +311,6 @@ def _norm_mag(x, mean, rstd, gamma, beta):
     return NORM * (rstd * gamma.to(D).abs() * (x.to(D).abs() + mean.abs()) + beta.to(D).abs())
 
 
-# The LayerNorm fold (lb_gemm ln_*, off by default) meets the LayerNorm-then-GEMM bound up to a row mean of 100 sigma.
-# At 256 sigma it does not (H100: 43 of 1 920 000 outputs over, worst 1.39 x the bound): ln_row_stats forms
-# E[x^2] - mu^2 from fp32 sums, the cancellation GroupNorm's statistics avoid with shifted sums (DESIGN section 4).
-@pytest.mark.parametrize("offset", [0.0, 10.0, 50.0, 100.0])
-def test_layernorm_fold_bound(offset):
-    """LayerNorm folded into the consuming GEMM, row statistics from the producing GEMM's stats_out, with row means
-    offset by ``offset`` sigma.  Bound: LayerNorm followed by the GEMM -- one ulp of each LayerNorm output and the
-    fp16 rounding of w * gamma (2^-10 + 2^-11 + ACC <= 2^-9 of sum |y||w|), NORM of the statistics times |w|, and one
-    ulp of the output."""
-    ops = _ops()
-    from latentblending_b200.unet import _fold_layernorm
-    M, C, N = 1000, 640, 1920
-    a, wp = _rand(M, C, seed=40), _rand(C, C, seed=41, s=0.3 * C ** -0.5)
-    res = _rand(M, C, seed=42, mean=offset)
-    parts = ops.gemm_stats_parts(a, wp, C, 1, 1, M)
-    stats = torch.zeros(M, parts, 2, dtype=torch.float32, device="cuda")
-    hs = ops.gemm(a, wp, C, 1, 1, M, res=res, stats_out=stats)
-    gamma, beta = _rand(C, seed=43, s=0.1, mean=1.0), _rand(C, seed=44, s=0.1)
-    w, b = _rand(N, C, seed=45, s=C ** -0.5), _rand(N, seed=46, s=0.1)
-    wf, csum, lnb = _fold_layernorm(w, b, gamma, beta)
-    out = ops.gemm(hs, wf, N, 1, 1, M, ln=dict(stats=stats, csum=csum, bias=lnb, eps=1e-5))
-    y, xh, mean, rstd = _ln_ref(hs, gamma, beta, 1e-5)
-    ref = y @ w.to(D).T + b.to(D)
-    wa = w.to(D).abs()
-    mag_y = ((xh * gamma.to(D)).abs() + beta.to(D).abs()) @ wa.T
-    bound = ULP * ref.abs() + P_TERM * mag_y + _norm_mag(hs, mean, rstd, gamma, beta) @ wa.T + TINY
-    check(out, ref, bound, f"LayerNorm fold, mean/sigma {offset}")
-    _flag_clear()
-
-
 # ---- attention -------------------------------------------------------------------------------------------------------
 _Q0, _K0, _V0, _O0 = 8, 64, 24, 16          # column of head 0 in each buffer (nonzero, different)
 

@@ -149,12 +149,6 @@ def test_bf16_gemm_rejections():
     w = _rand(256, 128, seed=22).to(BF)
     with pytest.raises(_cabi.LB200Error, match="GEGLU"):
         ops.gemm(a, w, 256, 1, 1, 256, mode=1)
-    st = torch.zeros(256, 32, 2, device="cuda")
-    with pytest.raises(_cabi.LB200Error, match="stats_out"):
-        ops.gemm(a, w, 256, 1, 1, 256, stats_out=st)
-    ln = dict(stats=st, csum=torch.zeros(256, device="cuda"), bias=torch.zeros(256, device="cuda"), eps=1e-5)
-    with pytest.raises(_cabi.LB200Error, match="LayerNorm"):
-        ops.gemm(a, w, 256, 1, 1, 256, ln=ln)
     with pytest.raises(_cabi.LB200Error, match="mixed"):
         ops.gemm(a.half(), w, 256, 1, 1, 256)
     with pytest.raises(_cabi.LB200Error, match="mixed"):
@@ -359,16 +353,6 @@ def test_bf16_decoder_at_1080p():
     assert frame.shape == (1080, 1920, 3)
     assert ops.error_flag() == 0 and vae.overflow_count() == 0
     assert frame.float().std() > 5
-
-
-def test_bf16_decoder_rejects_direct_conv_out(monkeypatch):
-    from latentblending_b200 import _cabi
-    from latentblending_b200.vae import VAEDecoderB200
-    ov, cfg = _tiny_upcast()
-    vae = VAEDecoderB200(ov.state_dict(), cfg.block_out_channels, cfg.scaling_factor, "cuda:0", dtype=BF)
-    monkeypatch.setenv("LB_CONV_OUT_DIRECT", "1")
-    with pytest.raises(_cabi.LB200Error, match="LB_CONV_OUT_DIRECT"):
-        vae.plan(8, 8)
 
 
 # ---- engine ----------------------------------------------------------------------------------------------------------
