@@ -272,7 +272,27 @@ int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, co
                const void* bias, int Cout, void* out, int64_t ldo, int act, float in_scale, void* stream, int dtype);
 int lb_upsample_nearest(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, int64_t ldo,
                         int Ho, int Wo, void* stream, int dtype);
+/* lb_conv_in_add: lb_conv_in (act 0, fp16) followed by the addition of a per-pixel addend shared by every image of
+ *   the batch: out row r = h(h(conv + bias) + addend[r mod H*W]) (h = fp16 rounding).  An SDXL ControlNet's
+ *   ``conv_in(x) + controlnet_cond_embedding(image)`` in one launch: the embedding [H*W, Cout] (row stride ld_add,
+ *   a multiple of 8) is computed once per control image and serves every batch row of every step. */
+int lb_conv_in_add(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                   const void* bias, int Cout, void* out, int64_t ldo, const void* addend, int64_t ld_add,
+                   void* stream);
 int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
+
+/* ---- ControlNet conditioning embedding (diffusers 0.25 ControlNetConditioningEmbedding) ----------------------
+ * lb_cond_conv: direct 3x3 convolution, zero padding 1, stride 1 or 2, of an NHWC map x [B*H*W rows, row stride
+ *   ld_x] into NHWC fp16 out [B*Ho*Wo, Cout] (row stride ldo), Ho = floor((H - 1) / stride) + 1 (likewise Wo);
+ *   fp32 accumulation, y = h(acc + bias), then y = h(silu(y)) when silu = 1 (h = fp16 rounding).  Weights are packed
+ *   [ky][kx][Cin][Cout] fp16.  in_u8 = 1: x is a uint8 image (1 to 8 channels, ld_x in bytes) and every input u is
+ *   read as h(u / 255) (the control image's VaeImageProcessor scaling, no normalisation to [-1, 1]); in_u8 = 0: x is
+ *   fp16 with Cin a multiple of 8 up to 256.  Cout a multiple of 8.  Meant for the small channel counts of the
+ *   embedding at full image resolution (3 -> 16 -> 32 -> 96 -> 256), where K = 9*Cin does not suit lb_gemm.
+ */
+int lb_cond_conv(lb_ctx* ctx, const void* x, int64_t ld_x, int B, int H, int W, int Cin, int in_u8,
+                 const void* w_packed, const void* bias, int Cout, int stride, int silu, void* out, int64_t ldo,
+                 void* stream);
 
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
  * lb_latent_prep: post_quant_conv(latents / scaling_factor) as a per-pixel CxC fp32 matrix (scale folded in).
@@ -337,12 +357,16 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * (diffusers_holder.py:336-344).
  * lb_op.dtype: the ``dtype`` argument of the record's call for the kinds whose entry point takes one (above); it must
  * be 0 for every other kind (a GEMM takes its types from its mode flags).  Kinds 8 and 18 are retired.
+ * LB_OP_CONV_IN_ADD (lb_conv_in_add) and LB_OP_COND_CONV (lb_cond_conv) use the ``conv`` member: CONV_IN_ADD reads
+ * x, B, Cin, H, W, w, bias, Cout, out, ld_out, addend, ld_add (act must be 0); COND_CONV reads x, ld_x, B, Cin, H, W,
+ * w, bias, Cout, out, ld_out, stride, in_u8 and act as lb_cond_conv's ``silu``.
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
     LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
-    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17
+    LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17,
+    LB_OP_CONV_IN_ADD = 19, LB_OP_COND_CONV = 20
 };
 typedef struct lb_op {
     int32_t kind;
@@ -357,9 +381,10 @@ typedef struct lb_op {
                  void* temb_in; void* add_in; } embed;
         struct { const void* x; int64_t ldx; int32_t M, K; const void* w; int64_t ldw; const void* bias;
                  const void* addend; int64_t ldadd; int32_t act_in, act_out; void* out; int64_t ldo; int32_t N; } lin;
-        /* CONV_IN (act, in_scale: lb_conv_in's) */
+        /* CONV_IN (act, in_scale: lb_conv_in's); CONV_IN_ADD and COND_CONV, see above */
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
-                 int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale; } conv;
+                 int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale;
+                 const void* addend; int64_t ld_add; int32_t stride, in_u8; } conv;
         /* UPSAMPLE_NEAREST: output Ho x Wo (see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
         struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; int32_t Ho, Wo; } resample;
         /* LATENT_PREP: x,w,bias,out,B,C,n=h*w; SOFTMAX_ROWS: x,ld_x,out,ld_out,n=rows,C=cols;

@@ -63,7 +63,8 @@ class _LinOp(ctypes.Structure):
 class _ConvOp(ctypes.Structure):
     _fields_ = [("x", c_void_p), ("ld_x", c_int64), ("B", c_int32), ("Cin", c_int32), ("H", c_int32), ("W", c_int32),
                 ("w", c_void_p), ("bias", c_void_p), ("Cout", c_int32), ("out", c_void_p), ("ld_out", c_int64),
-                ("act", c_int32), ("in_scale", c_float)]
+                ("act", c_int32), ("in_scale", c_float), ("addend", c_void_p), ("ld_add", c_int64),
+                ("stride", c_int32), ("in_u8", c_int32)]
 
 
 class _ResampleOp(ctypes.Structure):
@@ -103,6 +104,7 @@ DTYPE_F16, DTYPE_BF16 = 0, 1    # LB_DTYPE_F16 / LB_DTYPE_BF16: lb_op.dtype and 
 OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SMALL, OP_CONV_IN = 1, 2, 3, 4, 5, 6, 7
 (OP_UPSAMPLE_NEAREST, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
  OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = 9, 10, 11, 12, 13, 14, 15, 16, 17
+OP_CONV_IN_ADD, OP_COND_CONV = 19, 20
 CONV_IN_PLAIN, CONV_IN_TINY_VAE = 0, 1     # lb_conv_in's act
 
 
@@ -147,6 +149,10 @@ SIGNATURES = {
                                 c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_void_p]),
     "lb_conv_in": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                            c_int64, c_int, c_float, c_void_p, c_int]),
+    "lb_conv_in_add": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                               c_int64, c_void_p, c_int64, c_void_p]),
+    "lb_cond_conv": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                             c_int, c_int, c_void_p, c_int64, c_void_p]),
     "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
                                     c_int, c_void_p, c_int]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

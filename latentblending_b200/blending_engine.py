@@ -164,6 +164,13 @@ class BlendingEngine():
         self.parental_crossfeed_range = np.clip(crossfeed_range, 0, 1)
         self.parental_crossfeed_decay = np.clip(crossfeed_decay, 0, 1)
 
+    def set_control_image(self, image, conditioning_scale=1.0, guidance_start=0.0, guidance_end=1.0):
+        """Hold the transition's structure with the pipe's ControlNet: ``image`` (a PIL image or an HxWx3 uint8
+        array, e.g. a depth, canny or pose map) conditions every branch of the tree; ``None`` switches it off.
+        The arguments follow StableDiffusionXLControlNetPipeline's ``controlnet_conditioning_scale``,
+        ``control_guidance_start`` and ``control_guidance_end``.  Raises ValueError for a pipe without a ControlNet."""
+        self.dh.set_control_image(image, conditioning_scale, guidance_start, guidance_end)
+
     def set_prompt1(self, prompt: str):
         prompt = prompt.replace("_", " ")
         self.prompt1 = prompt

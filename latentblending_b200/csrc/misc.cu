@@ -118,10 +118,13 @@ __device__ __forceinline__ float tiny_vae_input(float v, float in_scale) {
     return lb_round_h(lb_round_h(tanhf(lb_round_h(z / 3.0f))) * 3.0f);
 }
 
-template <typename T, bool kTiny>
+// kAdd (lb_conv_in_add, fp16): out = h(h(conv + bias) + addend[pix mod H*W]) -- a ControlNet's
+// ``conv_in(x) + controlnet_cond_embedding(image)`` with one embedding row per pixel shared by every batch row.
+template <typename T, bool kTiny, bool kAdd = false>
 __device__ __forceinline__ void conv_in_body(const T* __restrict__ x, int B, int Cin, int H, int W,
                                              const T* __restrict__ wp, const T* __restrict__ bias, int Cout,
-                                             T* __restrict__ out, long long ldo, float in_scale) {
+                                             T* __restrict__ out, long long ldo, float in_scale,
+                                             const T* __restrict__ addend = nullptr, long long ld_add = 0) {
     using L = LbType<T>;
     pdl_launch_dependents();
     pdl_wait();
@@ -172,6 +175,16 @@ __device__ __forceinline__ void conv_in_body(const T* __restrict__ x, int B, int
 #pragma unroll
                 for (int j = 0; j < 8; ++j) acc[j] = fmaxf(acc[j], 0.f);
             }
+            if constexpr (kAdd) {
+                const uint4 av = *reinterpret_cast<const uint4*>(addend + (pix % ((long long)H * W)) * ld_add + g * 8);
+                const auto* ah = reinterpret_cast<const typename L::T2*>(&av);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 f = L::to_f2(ah[j]);
+                    acc[2 * j] = L::round(acc[2 * j]) + f.x;
+                    acc[2 * j + 1] = L::round(acc[2 * j + 1]) + f.y;
+                }
+            }
             uint4 o;
             auto* oh = reinterpret_cast<typename L::T2*>(&o);
 #pragma unroll
@@ -192,6 +205,13 @@ __global__ void __launch_bounds__(kThreads)
 conv_in_tiny_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const __half* __restrict__ wp,
                     const __half* __restrict__ bias, int Cout, __half* __restrict__ out, long long ldo, float in_scale) {
     conv_in_body<__half, true>(x, B, Cin, H, W, wp, bias, Cout, out, ldo, in_scale);
+}
+
+__global__ void __launch_bounds__(kThreads)
+conv_in_add_kernel(const __half* __restrict__ x, int B, int Cin, int H, int W, const __half* __restrict__ wp,
+                   const __half* __restrict__ bias, int Cout, __half* __restrict__ out, long long ldo,
+                   const __half* __restrict__ addend, long long ld_add) {
+    conv_in_body<__half, false, true>(x, B, Cin, H, W, wp, bias, Cout, out, ldo, 1.0f, addend, ld_add);
 }
 
 // ---- nearest upsample to Ho x Wo (Ho in {2H-1, 2H}, Wo in {2W-1, 2W}), NHWC ------------------------------------
@@ -332,6 +352,15 @@ extern "C" int lb_conv_in(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H
                                                                             Cout, out, ldo, stream);
     return conv_in_launch<__half, conv_in_kernel<__half>>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo,
                                                           stream);
+}
+
+extern "C" int lb_conv_in_add(lb_ctx* ctx, const void* x_nchw, int B, int Cin, int H, int W, const void* w_packed,
+                              const void* bias, int Cout, void* out, int64_t ldo, const void* addend, int64_t ld_add,
+                              void* stream) {
+    LB_REQUIRE(addend && ld_add >= Cout && ld_add % 8 == 0 && lb_aligned16(addend),
+               "lb_conv_in_add: addend needs a 16-byte aligned base and ld_add >= Cout, ld_add %% 8 == 0");
+    return conv_in_launch<__half, conv_in_add_kernel>(ctx, x_nchw, B, Cin, H, W, w_packed, bias, Cout, out, ldo,
+                                                      stream, (const __half*)addend, (long long)ld_add);
 }
 
 // the kernel moves 16-byte channel vectors, so fp16 and bf16 maps share it

@@ -97,6 +97,12 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
                 break;
+            case LB_OP_CONV_IN_ADD: case LB_OP_COND_CONV:
+                if (ops[i].kind == LB_OP_CONV_IN_ADD && ops[i].u.conv.act != 0) {
+                    lb_set_error("lb_program_create: op %lld: conv_in_add takes act 0", (long long)i);
+                    e = 2;
+                }
+                break;
             case LB_OP_CONV_IN: {
                 const auto& a = ops[i].u.conv;
                 if (a.act != 0 && a.act != 1) {
@@ -223,6 +229,18 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
                 const auto& a = o.u.conv;
                 e = lb_conv_in(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.act, a.in_scale,
                                stream, o.dtype);
+                break;
+            }
+            case LB_OP_CONV_IN_ADD: {
+                const auto& a = o.u.conv;
+                e = lb_conv_in_add(ctx, a.x, a.B, a.Cin, a.H, a.W, a.w, a.bias, a.Cout, a.out, a.ld_out, a.addend,
+                                   a.ld_add, stream);
+                break;
+            }
+            case LB_OP_COND_CONV: {
+                const auto& a = o.u.conv;
+                e = lb_cond_conv(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.Cin, a.in_u8, a.w, a.bias, a.Cout, a.stride, a.act,
+                                 a.out, a.ld_out, stream);
                 break;
             }
             case LB_OP_UPSAMPLE_NEAREST: {

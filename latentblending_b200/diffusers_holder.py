@@ -47,7 +47,14 @@ class DiffusersHolder:
         s = pipe.unet_cfg.sample_size
         self.width_latent = self.height_latent = s
         self.width_img = self.height_img = s * pipe.vae_scale_factor
-        self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device)
+        # an SDXL ControlNet (pipe.controlnet of a StableDiffusionXLControlNetPipeline): lowered into every UNet plan
+        # as a second step program, run while a control image is set (set_control_image)
+        self.controlnet, self.control = None, None
+        if getattr(pipe, "controlnet_state_dict", None) is not None:
+            from .controlnet import COND_CHANNELS, ControlNetB200
+            self.controlnet = ControlNetB200(pipe.controlnet_cfg, pipe.controlnet_state_dict, self.device,
+                                             getattr(pipe, "controlnet_cond_channels", None) or COND_CHANNELS)
+        self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device, controlnet=self.controlnet)
         self.vae = None
         self.set_vae_dtype(getattr(pipe, "vae_dtype", "fp16"))
         self.noise_fn = None          # tests: inject the ancestral-step noise, noise_fn(i, shape)
@@ -98,6 +105,56 @@ class DiffusersHolder:
         self.width_latent = int(self.width_img / s)
         self.height_img = int(round(height / s) * s)
         self.height_latent = int(self.height_img / s)
+        if self.control is not None:
+            self._embed_control(self.height_latent, self.width_latent)
+
+    def set_control_image(self, image, conditioning_scale=1.0, guidance_start=0.0, guidance_end=1.0):
+        """Condition every following denoise on ``image`` (a PIL image or an HxWx3 uint8 array) through the pipe's
+        ControlNet; ``None`` switches the ControlNet off.  The arguments are StableDiffusionXLControlNetPipeline's
+        ``controlnet_conditioning_scale``, ``control_guidance_start`` and ``control_guidance_end``: the ControlNet's
+        residuals, times ``conditioning_scale``, are added at the steps i of N with start <= i/N and
+        (i+1)/N <= end.  The image is converted to RGB and resized with LANCZOS to the output size, as the
+        pipeline's control image processor does, and embedded once per image and size."""
+        if self.controlnet is None:
+            raise ValueError("set_control_image needs a pipe with a ControlNet (StableDiffusionXLControlNetPipeline, "
+                             "or SyntheticSDXLPipe(controlnet=...))")
+        if image is None:
+            self.control = None
+            return
+        if not (0.0 <= guidance_start < guidance_end <= 1.0):
+            raise ValueError(f"need 0 <= guidance_start < guidance_end <= 1 (got {guidance_start}, {guidance_end})")
+        from PIL import Image
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+                raise ValueError(f"a control image array must be HxWx3 uint8 (got {image.dtype} {image.shape})")
+            image = Image.fromarray(image)
+        elif not isinstance(image, Image.Image):
+            raise TypeError(f"the control image must be a PIL image or an HxWx3 uint8 array (got {type(image)})")
+        self.controlnet.set_scale(conditioning_scale)
+        self.control = dict(image=image.convert("RGB"), scale=float(conditioning_scale), start=float(guidance_start),
+                            end=float(guidance_end), embedded=set())
+        self._embed_control(self.height_latent, self.width_latent)
+
+    def _embed_control(self, h, w):
+        """Fill the ControlNet's conditioning embedding for latent size (h, w) unless the current image already is."""
+        c = self.control
+        if (h, w) in c["embedded"]:
+            return
+        from PIL import Image
+        s = self.pipe.vae_scale_factor
+        arr = np.array(c["image"].resize((w * s, h * s), resample=Image.LANCZOS))
+        if getattr(self.pipe, "controlnet_bgr", False):
+            arr = arr[:, :, ::-1]
+        self.controlnet.embed(torch.from_numpy(np.ascontiguousarray(arr)).to(self.device), h, w)
+        c["embedded"].add((h, w))
+
+    def control_active(self, i, num_steps):
+        """Whether step ``i`` of ``num_steps`` runs the UNet + ControlNet step program (else the plain one)."""
+        c = self.control
+        if c is None:
+            return False
+        from .controlnet import keep_scale
+        return keep_scale(i, num_steps, c["start"], c["end"]) * c["scale"] > 0
 
     def set_negative_prompt(self, negative_prompt):
         self.negative_prompt = [negative_prompt] if isinstance(negative_prompt, str) else negative_prompt
@@ -236,6 +293,8 @@ class DiffusersHolder:
             eps_pair = self._eps_pair[key]
         if dual is None:
             plan.prog_ctx.run()                                # cross-attention K/V: once per conditioning
+        if self.control is not None:
+            self._embed_control(h, w)
         n = C * h * w
         outs = [[None] * N for _ in jobs]
         trajs = [torch.empty((N, C, h, w), dtype=torch.float16, device=self.device) for _ in jobs]
@@ -278,15 +337,16 @@ class DiffusersHolder:
                     scaled[j] = False
                 if not scaled[j]:
                     ops.scale_model_input(latents[j], Bj, sc["divisor"], out=x_in[j * Bj:(j + 1) * Bj])
+            control = self.control_active(i, N)
             if dual is None:
-                plan.prog_step.run(sc["t"])
+                (plan.prog_step_cn if control else plan.prog_step).run(sc["t"])
             else:
                 main = torch.cuda.current_stream()
                 dual["fork"].record(main)
                 for pl, st, ev in zip(dual["plans"], dual["streams"], dual["done"]):
                     st.wait_event(dual["fork"])
                     with torch.cuda.stream(st):
-                        pl.prog_step.run(sc["t"])
+                        (pl.prog_step_cn if control else pl.prog_step).run(sc["t"])
                         ev.record(st)
                 for ev in dual["done"]:
                     main.wait_event(ev)

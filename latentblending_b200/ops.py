@@ -267,6 +267,27 @@ def conv_in(x_nchw, w_packed, bias, Cout, out=None, act=_cabi.CONV_IN_PLAIN, in_
     return out
 
 
+def conv_in_add(x_nchw, w_packed, bias, Cout, addend, out=None):
+    """fp16 ``conv_in`` plus ``addend`` [H*W, >=Cout], added to every image of the batch (lb_conv_in_add)."""
+    dev = _dev(x_nchw)
+    B, _, H, W = x_nchw.shape
+    if out is None:
+        out = torch.empty((B * H * W, Cout), dtype=torch.float16, device=x_nchw.device)
+    _run1(dev, lambda P: P.conv_in_add(x_nchw, w_packed, bias, Cout, out, addend))
+    return out
+
+
+def cond_conv(x, B, H, W, Cin, w_packed, bias, Cout, stride=1, silu=False, out=None):
+    """Direct 3x3 pad-1 conv (lb_cond_conv) of NHWC fp16 rows or a uint8 image [B*H*W, Cin] -> fp16
+    [B*Ho*Wo, Cout], Ho = ceil(H / stride)."""
+    dev = _dev(x)
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    if out is None:
+        out = torch.empty((B * Ho * Wo, Cout), dtype=torch.float16, device=x.device)
+    _run1(dev, lambda P: P.cond_conv(x, B, H, W, Cin, w_packed, bias, Cout, out, stride=stride, silu=silu))
+    return out
+
+
 def conv_out(x, B, H, W, Cin, w_packed, bias, Cout, out=None):
     """The Cin -> Cout 3x3 output convolution of NHWC ``x`` into NCHW, as the lowerings run it: ``w_packed``
     [Cout][3][3][Cin] through ``pack_conv_out8``, then ``Program.conv_out_gemm``."""

@@ -121,6 +121,52 @@ def unet_param_shapes(cfg: UNetConfig):
     return P
 
 
+def controlnet_param_shapes(cfg: UNetConfig, cond_channels=None):
+    """diffusers state_dict names -> shapes of an SDXL ControlNetModel whose encoder is ``cfg`` (its own transformer
+    depths): the UNet's conv_in, embeddings, down and mid blocks, the conditioning embedding
+    (``controlnet_cond_embedding``) and the zero convs (``controlnet_down_blocks.{i}``, ``controlnet_mid_block``)."""
+    from .controlnet import COND_CHANNELS, cond_embedding_layers, num_down_residuals
+    cond_channels = COND_CHANNELS if cond_channels is None else tuple(cond_channels)
+    P = OrderedDict((k, v) for k, v in unet_param_shapes(cfg).items()
+                    if not k.startswith(("up_blocks.", "conv_norm_out.", "conv_out.", "mid_block.")))
+    for name, cin, cout, _, _ in cond_embedding_layers(cond_channels, cfg.block_out_channels[0]):
+        P[name + ".weight"], P[name + ".bias"] = (cout, cin, 3, 3), (cout,)
+    L, ch = len(cfg.block_out_channels), cfg.block_out_channels
+    chans = [ch[0]]
+    for i in range(L):
+        chans += [ch[i]] * cfg.layers_per_block + ([ch[i]] if i < L - 1 else [])
+    assert len(chans) == num_down_residuals(cfg)
+    for i, c in enumerate(chans):
+        P[f"controlnet_down_blocks.{i}.weight"], P[f"controlnet_down_blocks.{i}.bias"] = (c, c, 1, 1), (c,)
+    P.update((k, v) for k, v in unet_param_shapes(cfg).items() if k.startswith("mid_block."))
+    P["controlnet_mid_block.weight"], P["controlnet_mid_block.bias"] = (ch[-1], ch[-1], 1, 1), (ch[-1],)
+    return P
+
+
+def controlnet_config(unet_cfg: UNetConfig, variant):
+    """The encoder config of SyntheticSDXLPipe's ControlNet: "full" keeps the UNet's transformer depths (as
+    diffusers/controlnet-canny-sdxl-1.0 does), "small" has one transformer block, in the mid block's level only."""
+    import dataclasses
+    L = len(unet_cfg.block_out_channels)
+    if variant == "full":
+        depths = tuple(unet_cfg.transformer_layers)
+    elif variant == "small":
+        depths = (0,) * (L - 1) + (1,)
+    else:
+        raise ValueError(f"controlnet must be None, 'full' or 'small' (got {variant!r})")
+    return dataclasses.replace(unet_cfg, transformer_layers=depths, time_cond_proj_dim=None)
+
+
+def random_controlnet_state_dict(cfg: UNetConfig, seed, device, damp=0.1):
+    """Seeded ControlNet weights with ``random_state_dict``'s recipe.  The zero convs are damped like the other
+    residual branches but not zero, so the control branch changes the UNet's output."""
+    sd = random_state_dict(controlnet_param_shapes(cfg), seed, device, damp=damp)
+    for k in sd:
+        if k.startswith(("controlnet_down_blocks.", "controlnet_mid_block.")):
+            sd[k] = (sd[k].float() * damp).to(sd[k].dtype)
+    return sd
+
+
 def vae_param_shapes(channels=VAE_CHANNELS, latent=4):
     P = OrderedDict()
     ch = list(reversed(channels))
@@ -257,7 +303,8 @@ class SyntheticSDXLPipe:
 
     def __init__(self, name="stabilityai/stable-diffusion-xl-base-1.0", device="cuda:0", unet_cfg: UNetConfig = None,
                  seed=0, unet_state_dict=None, vae_state_dict=None, vae_channels=VAE_CHANNELS,
-                 lpips_state_dict=None, vae_dtype="fp16", vae="kl", scheduler=None):
+                 lpips_state_dict=None, vae_dtype="fp16", vae="kl", scheduler=None, controlnet=None,
+                 controlnet_state_dict=None):
         """``scheduler``: None (Euler for SDXL base, Euler-ancestral for a name with "turbo"), "euler",
         "euler_ancestral", "lcm" (LCMScheduler tables: LCM-LoRA-style with the base UNet, LCM-SDXL-style with
         ``unet_cfg.time_cond_proj_dim`` set) or one of DPM_SCHEDULERS (DPMSolverMultistepScheduler tables for the SDXL
@@ -265,7 +312,9 @@ class SyntheticSDXLPipe:
         ``vae_dtype``: "fp16" or "bf16", the storage type of the VAE decoder DiffusersHolder builds.
         ``vae``: "kl" (the SDXL AutoencoderKL decoder) or "tiny" (the AutoencoderTiny / TAESDXL decoder with its
         default config, scaling_factor 1.0, fp16 only; ``vae_state_dict`` then holds its ``decoder.``-stripped
-        weights, seeded by ``random_tiny_vae_state_dict`` when omitted)."""
+        weights, seeded by ``random_tiny_vae_state_dict`` when omitted).
+        ``controlnet``: None, "full" or "small" (``controlnet_config``): an SDXL ControlNet with seeded weights
+        (``random_controlnet_state_dict``) unless ``controlnet_state_dict`` is given."""
         if vae_dtype not in VAE_DTYPES:
             raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
         if vae not in ("kl", "tiny"):
@@ -305,6 +354,13 @@ class SyntheticSDXLPipe:
         self.vae_dtype = vae_dtype
         self.lpips_state_dict = lpips_state_dict
         self.h2d_bytes = 0        # bytes of conditioning copied host->device (bench e2e)
+        self.controlnet_cfg = self.controlnet_state_dict = None
+        if controlnet is not None:
+            self.controlnet_cfg = controlnet_config(self.unet_cfg, controlnet)
+            self.controlnet_state_dict = controlnet_state_dict if controlnet_state_dict is not None else \
+                random_controlnet_state_dict(self.controlnet_cfg, seed + 2, self.device)
+        self.controlnet_cond_channels = None          # the default, controlnet.COND_CHANNELS
+        self.controlnet_bgr = False
 
     def encode_prompt(self, prompt, negative_prompt=None, do_classifier_free_guidance=True, dtype=torch.float16):
         """Synthetic stand-in for StableDiffusionXLPipeline.encode_prompt (diffusers_holder.py:81-95)."""
@@ -324,6 +380,37 @@ class SyntheticSDXLPipe:
         neg = negative_prompt[0] if isinstance(negative_prompt, (list, tuple)) else (negative_prompt or "")
         ne, npool = emb("<neg>" + neg)
         return pe, ne, pp, npool
+
+
+def _sdxl_encoder_config(ucfg, what, defaults=None):
+    """The UNetConfig of a diffusers SDXL UNet2DConditionModel or ControlNetModel config (``what`` names it in errors);
+    keys the config lacks (a ControlNet has no out_channels or sample_size) come from ``defaults``."""
+
+    def get(k, default=None):
+        if k in ucfg:
+            return ucfg[k]
+        return getattr(ucfg, k, getattr(defaults, k, default) if defaults is not None else default)
+    tl = get("transformer_layers_per_block", 1)
+    down = list(get("down_block_types"))
+    boc = tuple(get("block_out_channels"))
+    if isinstance(tl, int):
+        tl = [tl] * len(boc)
+    tl = tuple(int(t) if "CrossAttn" in d else 0 for t, d in zip(tl, down))
+    ahd = get("attention_head_dim")
+    heads = ahd if isinstance(ahd, (list, tuple)) else [ahd] * len(boc)
+    # SDXL's config stores the number of heads per level in attention_head_dim (5, 10, 20): head dim = C / heads
+    head_dims = {c // h for c, h, t in zip(boc, heads, tl) if t}
+    if head_dims != {64}:
+        raise ValueError(f"this backend implements head dim 64 (SDXL); the pipeline's {what} has {sorted(head_dims)}")
+    if get("addition_embed_type") != "text_time" or not get("use_linear_projection", False):
+        raise ValueError(f"not an SDXL {what} (needs addition_embed_type='text_time', use_linear_projection=True)")
+    pooled = int(get("projection_class_embeddings_input_dim")) - 6 * int(get("addition_time_embed_dim"))
+    return UNetConfig(in_channels=get("in_channels"), out_channels=get("out_channels"),
+                      block_out_channels=boc, layers_per_block=get("layers_per_block"),
+                      transformer_layers=tl, head_dim=64, cross_attention_dim=get("cross_attention_dim"),
+                      addition_time_embed_dim=get("addition_time_embed_dim"), pooled_dim=pooled,
+                      norm_num_groups=get("norm_num_groups"), sample_size=get("sample_size"),
+                      time_cond_proj_dim=get("time_cond_proj_dim"))
 
 
 class DiffusersSDXLPipe:
@@ -355,31 +442,7 @@ class DiffusersSDXLPipe:
         self._name_or_path = getattr(pipe, "_name_or_path", None) or pipe.config.get("_name_or_path", "")
         self._execution_device = torch.device(pipe._execution_device)
         self.device = self._execution_device
-        ucfg = pipe.unet.config
-
-        def get(k, default=None):
-            return ucfg[k] if k in ucfg else getattr(ucfg, k, default)
-        tl = get("transformer_layers_per_block", 1)
-        down = list(get("down_block_types"))
-        boc = tuple(get("block_out_channels"))
-        if isinstance(tl, int):
-            tl = [tl] * len(boc)
-        tl = tuple(int(t) if "CrossAttn" in d else 0 for t, d in zip(tl, down))
-        ahd = get("attention_head_dim")
-        heads = ahd if isinstance(ahd, (list, tuple)) else [ahd] * len(boc)
-        # SDXL's config stores the number of heads per level in attention_head_dim (5, 10, 20): head dim = C / heads
-        head_dims = {c // h for c, h, t in zip(boc, heads, tl) if t}
-        if head_dims != {64}:
-            raise ValueError(f"this backend implements head dim 64 (SDXL); the pipeline's UNet has {sorted(head_dims)}")
-        if get("addition_embed_type") != "text_time" or not get("use_linear_projection", False):
-            raise ValueError("not an SDXL UNet (needs addition_embed_type='text_time', use_linear_projection=True)")
-        pooled = int(get("projection_class_embeddings_input_dim")) - 6 * int(get("addition_time_embed_dim"))
-        self.unet_cfg = UNetConfig(in_channels=get("in_channels"), out_channels=get("out_channels"),
-                                   block_out_channels=boc, layers_per_block=get("layers_per_block"),
-                                   transformer_layers=tl, head_dim=64, cross_attention_dim=get("cross_attention_dim"),
-                                   addition_time_embed_dim=get("addition_time_embed_dim"), pooled_dim=pooled,
-                                   norm_num_groups=get("norm_num_groups"), sample_size=get("sample_size"),
-                                   time_cond_proj_dim=get("time_cond_proj_dim"))
+        self.unet_cfg = _sdxl_encoder_config(pipe.unet.config, "UNet")
         self.default_sample_size = getattr(pipe, "default_sample_size", self.unet_cfg.sample_size)
         self.vae_scale_factor = pipe.vae_scale_factor
         self.scheduler = tables_from_diffusers_scheduler(pipe.scheduler)
@@ -388,6 +451,7 @@ class DiffusersSDXLPipe:
         if lora:
             raise ValueError(f"the pipeline's UNet holds unfused LoRA layers ({len(lora)} keys, e.g. {lora[0]!r}): "
                              "fuse them into the weights first with pipe.fuse_lora(); pipe.unload_lora_weights()")
+        self._take_controlnet(getattr(pipe, "controlnet", None))
         vsd = pipe.vae.state_dict()
         vcfg = pipe.vae.config
         if type(pipe.vae).__name__ == "AutoencoderTiny":
@@ -411,6 +475,51 @@ class DiffusersSDXLPipe:
             self.vae_dtype = vae_dtype_from_config(vcfg)
         self.lpips_state_dict = lpips_state_dict if lpips_state_dict is not None else getattr(pipe, "lpips_state_dict", None)
         self.h2d_bytes = 0
+
+    def _take_controlnet(self, cn):
+        """A StableDiffusionXLControlNetPipeline's ``controlnet`` (one ControlNetModel): its encoder config, the
+        conditioning embedding's channels and channel order, and its state dict, every key of which the lowering
+        must represent."""
+        self.controlnet_cfg = self.controlnet_state_dict = self.controlnet_cond_channels = None
+        self.controlnet_bgr = False
+        if cn is None:
+            return
+        if type(cn).__name__ == "MultiControlNetModel" or isinstance(cn, (list, tuple)):
+            raise ValueError("several ControlNets at once (MultiControlNetModel) are not supported")
+        c = cn.config
+
+        def get(k, default=None):
+            return c[k] if k in c else getattr(c, k, default)
+        if get("global_pool_conditions", False):
+            raise ValueError("a ControlNet with global_pool_conditions=True is not supported")
+        if get("conditioning_channels", 3) != 3:
+            raise ValueError(f"the ControlNet takes {get('conditioning_channels')} conditioning channels; only 3 (an "
+                             "RGB control image) are supported")
+        if get("time_cond_proj_dim") is not None:
+            raise ValueError("a ControlNet with time_embedding.cond_proj (time_cond_proj_dim) is not supported")
+        order = get("controlnet_conditioning_channel_order", "rgb")
+        if order not in ("rgb", "bgr"):
+            raise ValueError(f"unknown controlnet_conditioning_channel_order {order!r}")
+        ccfg = _sdxl_encoder_config(c, "ControlNet", defaults=self.unet_cfg)
+        u = self.unet_cfg
+        for f in ("in_channels", "block_out_channels", "layers_per_block", "cross_attention_dim",
+                  "addition_time_embed_dim", "pooled_dim", "norm_num_groups"):
+            if getattr(ccfg, f) != getattr(u, f):
+                raise ValueError(f"the ControlNet's encoder does not match the UNet's: {f} {getattr(ccfg, f)} vs "
+                                 f"{getattr(u, f)}")
+        cond = tuple(get("conditioning_embedding_out_channels", (16, 32, 96, 256)))
+        sd = cn.state_dict()
+        want = controlnet_param_shapes(ccfg, cond)
+        extra, missing = sorted(set(sd) - set(want)), sorted(set(want) - set(sd))
+        if extra or missing:
+            raise ValueError(f"the ControlNet's layout is not one this lowering represents: {len(extra)} unexpected "
+                             f"keys (e.g. {extra[:3]}), {len(missing)} missing (e.g. {missing[:3]})")
+        bad = [k for k, shp in want.items() if tuple(sd[k].shape) != shp]
+        if bad:
+            raise ValueError(f"the ControlNet's parameter shapes differ from its config's, e.g. {bad[0]!r}: "
+                             f"{tuple(sd[bad[0]].shape)} vs {want[bad[0]]}")
+        self.controlnet_cfg, self.controlnet_state_dict = ccfg, sd
+        self.controlnet_cond_channels, self.controlnet_bgr = cond, order == "bgr"
 
     def encode_prompt(self, prompt, negative_prompt=None, do_classifier_free_guidance=True, dtype=torch.float16):
         """diffusers_holder.py:79-96: the pipeline's own encode_prompt (both CLIP encoders), 4-tuple out."""

@@ -7,7 +7,8 @@ import ctypes
 import torch
 
 from . import _cabi
-from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_CONV_IN, OP_EMBED_INPUTS, OP_GEMM,
+from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_COND_CONV, OP_CONV_IN, OP_CONV_IN_ADD,
+                    OP_EMBED_INPUTS, OP_GEMM,
                     OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
                     OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS,
                     OP_UPSAMPLE_NEAREST, Op, check, ctx, stream_ptr)
@@ -171,6 +172,30 @@ class Program:
         d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
         d.out, d.ld_out, d.act, d.in_scale = _p(out), out.stride(0), int(act), float(in_scale)
         self.hold(x_nchw, w, bias, out)
+
+    def conv_in_add(self, x_nchw, w, bias, Cout, out, addend):
+        """fp16 ``conv_in`` then ``+ addend[r mod H*W]`` (lb_conv_in_add): a ControlNet's conv_in(x) plus the
+        conditioning embedding [H*W, Cout] every batch row shares."""
+        _same_dtype(torch.float16, "conv_in_add x / w / bias / out / addend", x_nchw, w, bias, out, addend)
+        d = self._new(OP_CONV_IN_ADD).u.conv
+        B, Cin, H, W = x_nchw.shape
+        if addend.shape[0] != H * W:
+            raise _cabi.LB200Error(f"conv_in_add: the addend has {addend.shape[0]} rows, the map {H}x{W} pixels")
+        d.x, d.B, d.Cin, d.H, d.W, d.w, d.bias, d.Cout = _p(x_nchw), B, Cin, H, W, _p(w), _p(bias), Cout
+        d.out, d.ld_out, d.addend, d.ld_add = _p(out), out.stride(0), _p(addend), addend.stride(0)
+        self.hold(x_nchw, w, bias, out, addend)
+
+    def cond_conv(self, x, B, H, W, Cin, w, bias, Cout, out, stride=1, silu=False):
+        """Direct 3x3 pad-1 conv of NHWC ``x`` (fp16 [B*H*W, >=Cin], or a uint8 image read as u / 255) into fp16
+        ``out`` [B*Ho*Wo, >=Cout] (lb_cond_conv); ``w`` packed [ky][kx][Cin][Cout]."""
+        if x.dtype not in (torch.uint8, torch.float16):
+            raise _cabi.LB200Error(f"cond_conv: x must be uint8 or float16 (got {x.dtype})")
+        _same_dtype(torch.float16, "cond_conv w / bias / out", w, bias, out)
+        d = self._new(OP_COND_CONV).u.conv
+        d.x, d.ld_x, d.B, d.Cin, d.H, d.W = _p(x), x.stride(-2), B, Cin, H, W
+        d.w, d.bias, d.Cout, d.out, d.ld_out = _p(w), _p(bias), Cout, _p(out), out.stride(0)
+        d.act, d.stride, d.in_u8 = int(silu), stride, int(x.dtype == torch.uint8)
+        self.hold(x, w, bias, out)
 
     def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp):
         """The C0 -> Cout (<= 8) 3x3 output convolution on the tensor-core GEMM: N = 8 (zero-padded weight rows),

@@ -80,12 +80,24 @@ class PackedUNet:
     """fp16 device copies of the UNet parameters in the layouts the kernels consume."""
 
     def __init__(self, cfg: UNetConfig, state_dict, device):
+        self._pack_encoder(cfg, state_dict, device)
+        W, g = self.w, self.g
+        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(g("conv_out.weight").permute(0, 2, 3, 1),
+                                                            g("conv_out.bias"))
+        for nm in ("conv_norm_out",):
+            W[nm + ".g"], W[nm + ".b"] = g(nm + ".weight"), g(nm + ".bias")
+
+    def _pack_encoder(self, cfg, state_dict, device):
+        """What a UNet shares with a ControlNet: conv_in, the time / added-condition embeddings, every resnet (with
+        the stacked time_emb_proj), transformer and resampler.  ``self.consumed``: the state-dict names read."""
         self.cfg = cfg
         self.device = torch.device(device)
         sd = state_dict
         dev = self.device
+        self.consumed = set()
 
         def g(name):
+            self.consumed.add(name)
             return sd[name].detach().to(device=dev, dtype=torch.float16).contiguous()
 
         self.g = g
@@ -93,10 +105,6 @@ class PackedUNet:
         W = self.w
         W["conv_in.w"] = g("conv_in.weight").permute(2, 3, 1, 0).contiguous()      # [ky][kx][cin][Cout]
         W["conv_in.b"] = g("conv_in.bias")
-        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(g("conv_out.weight").permute(0, 2, 3, 1),
-                                                            g("conv_out.bias"))
-        for nm in ("conv_norm_out",):
-            W[nm + ".g"], W[nm + ".b"] = g(nm + ".weight"), g(nm + ".bias")
         for e in ("time_embedding", "add_embedding"):
             for l in ("linear_1", "linear_2"):
                 W[f"{e}.{l}.w"], W[f"{e}.{l}.b"] = g(f"{e}.{l}.weight"), g(f"{e}.{l}.bias")
@@ -160,11 +168,14 @@ class PackedUNet:
 class UNetB200:
     """One lowered forward per (batch, h, w); ``forward`` replays it."""
 
-    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0"):
+    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0", controlnet=None):
+        """``controlnet``: a ``controlnet.ControlNetB200`` on the same device; every plan then also records
+        ``prog_step_cn``, the step with the ControlNet's residuals added."""
         self.cfg = cfg
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
         self.packed = PackedUNet(cfg, state_dict, self.device)
+        self.controlnet = controlnet
         self._plans = {}
 
     # -- public -----------------------------------------------------------------------------
@@ -177,9 +188,12 @@ class UNetB200:
         return self._plans[key]
 
     @torch.no_grad()
-    def forward(self, x, t, encoder_hidden_states, text_embeds, time_ids, ctx_changed=True, timestep_cond=None):
+    def forward(self, x, t, encoder_hidden_states, text_embeds, time_ids, ctx_changed=True, timestep_cond=None,
+                control=False):
         """x [B,4,h,w] fp16 NCHW -> eps [B,4,h,w] fp16 (a view of the plan's static output buffer).
-        ``timestep_cond`` [B, time_cond_proj_dim]: the guidance-scale embedding a time-conditioned UNet requires."""
+        ``timestep_cond`` [B, time_cond_proj_dim]: the guidance-scale embedding a time-conditioned UNet requires.
+        ``control``: add the attached ControlNet's residuals (its conditioning embedding for (h, w) as last
+        filled by ``ControlNetB200.embed``, its scale as last set)."""
         B, _, H, W = x.shape
         pl = self.plan(B, H, W)
         if (pl.wcond is None) != (timestep_cond is None):
@@ -192,7 +206,9 @@ class UNetB200:
         if ctx_changed:
             pl.ctx.copy_(encoder_hidden_states.reshape(pl.ctx.shape))
             pl.prog_ctx.run()
-        pl.prog_step.run(float(t))
+        if control and pl.prog_step_cn is None:
+            raise ValueError("control=True needs a UNetB200 built with a controlnet")
+        (pl.prog_step_cn if control else pl.prog_step).run(float(t))
         return pl.eps
 
     def launches_per_forward(self, B, H, W):
@@ -208,7 +224,6 @@ class _Lowering:
         f16 = dict(dtype=torch.float16, device=dev)
         ch = list(cfg.block_out_channels)
         L = len(ch)
-        T = cfg.time_embed_dim
         groups = cfg.norm_num_groups
         if x_in is not None:
             assert tuple(x_in.shape) == (B, cfg.in_channels, H, W) and x_in.dtype == torch.float16 and x_in.is_contiguous()
@@ -231,30 +246,28 @@ class _Lowering:
             t = torch.empty(rows, cols, **f16)
             self._persist.append(t)
             return t
+        self.persist, self.scratch = persist, scratch
 
         # ---- embeddings -------------------------------------------------------------------
         temb_in, add_in = persist(B, ch[0]), persist(B, cfg.add_in_dim)
         P.embed_inputs(self.text, self.tids, ch[0], cfg.addition_time_embed_dim, temb_in, add_in)
+        self.temb_in, self.add_in = temb_in, add_in         # the sinusoid features; a ControlNet embeds them too
         if self.wcond is not None:        # TimestepEmbedding: sample + cond_proj(condition), then linear_1
             tc_in = persist(B, ch[0])
             P.linear_small(self.wcond, Wt["time_embedding.cond_proj.w"], tc_in, addend=temb_in)
             temb_in = tc_in
-        t1, a1, temb, emb = persist(B, T), persist(B, T), persist(B, T), persist(B, T)
-        P.linear_small(temb_in, Wt["time_embedding.linear_1.w"], t1, bias=Wt["time_embedding.linear_1.b"], act_out=1)
-        P.linear_small(t1, Wt["time_embedding.linear_2.w"], temb, bias=Wt["time_embedding.linear_2.b"])
-        P.linear_small(add_in, Wt["add_embedding.linear_1.w"], a1, bias=Wt["add_embedding.linear_1.b"], act_out=1)
-        P.linear_small(a1, Wt["add_embedding.linear_2.w"], emb, bias=Wt["add_embedding.linear_2.b"], addend=temb)
-        temb_all = persist(B, net.packed.temb_total)
-        P.linear_small(emb, Wt["temb_all.w"], temb_all, bias=Wt["temb_all.b"], act_in=1)
+        temb_all = self.embed(P, net.packed, temb_in)
 
         # ---- geometry + concat buffers ------------------------------------------------------
         # the stride-2 pad-1 Downsample2D conv gives ceil(s/2); the up path resizes back to each skip level's size
         res_hw = [(H, W)]
         for _ in range(L - 1):
             res_hw.append(((res_hw[-1][0] + 1) // 2, (res_hw[-1][1] + 1) // 2))
+        self.res_hw = res_hw
 
         def rows_at(level):
             return B * res_hw[level][0] * res_hw[level][1]
+        self.rows_at = rows_at
 
         # skip list: (level, channels) in production order
         skip_meta = [(0, ch[0])]
@@ -262,6 +275,7 @@ class _Lowering:
             skip_meta += [(i, ch[i])] * cfg.layers_per_block
             if i < L - 1:
                 skip_meta.append((i + 1, ch[i]))
+        self.skip_meta = skip_meta
         # up path consumption: resnet j of up block i
         rev = list(reversed(ch))
         cats = []              # in pop order
@@ -276,21 +290,21 @@ class _Lowering:
                 cats.append(dict(buf=buf, hidden=buf[:, :hidden_c], skip=buf[:, hidden_c:], level=lvl))
                 k -= 1
             cprev = cout
+        self.cats = cats
         skip_views = [c["skip"] for c in reversed(cats)]      # index by production order
+        self.skip_views = skip_views
+        unet = dict(W=Wt, packed=net.packed, temb_all=temb_all, depths=cfg.transformer_layers)
 
-        def tslice(rname):
-            off, n = net.packed.temb_off[rname]
-            return temb_all[:, off:off + n]
-
-        def resnet(rname, x, cin, cout, level, out):
+        def resnet(P, prm, rname, x, cin, cout, level, out):
             h_, w_ = res_hw[level]
-            lower_resnet(P, Wt, rname, x, cin, cout, B, h_, w_, out, groups, 1e-5, self.ws, scratch, bias2=tslice(rname))
-
-        kv_cache = {}
+            off, n = prm["packed"].temb_off[rname]
+            lower_resnet(P, prm["W"], rname, x, cin, cout, B, h_, w_, out, groups, 1e-5, self.ws, scratch,
+                         bias2=prm["temb_all"][:, off:off + n])
 
         geglu_mode = 1
 
-        def transformer(aname, x, C, level, out):
+        def transformer(P, prm, aname, x, C, level, out):
+            Wt = prm["W"]
             h_, w_ = res_hw[level]
             S = h_ * w_
             M = rows_at(level)
@@ -307,7 +321,6 @@ class _Lowering:
                 gg = scratch("geglu", M, 4 * C)
                 kv = persist(B * 77, 2 * C)         # depends on the conditioning only: computed by prog_ctx
                 PC.gemm(self.ctx, Wt[t + ".attn2.kv.w"], 2 * C, 1, 1, B * 77, kv)
-                kv_cache[t] = kv
                 ln = scratch("ln", M, C)
                 P.layernorm(hs, Wt[t + ".norm1.g"], Wt[t + ".norm1.b"], 1e-5, ln)
                 P.gemm(ln, Wt[t + ".attn1.qkv.w"], 3 * C, 1, 1, M, qkv)
@@ -322,40 +335,48 @@ class _Lowering:
                 P.gemm(gg, Wt[t + ".ff.out.w"], C, 1, 1, M, hs, bias=Wt[t + ".ff.out.b"], res=hs)
             P.gemm(hs, Wt[aname + ".proj_out.w"], C, 1, 1, M, out, bias=Wt[aname + ".proj_out.b"], res=x)
 
-        # ---- down path ----------------------------------------------------------------------
-        si = 0
-        P.conv_in(self.x_in, Wt["conv_in.w"], Wt["conv_in.b"], ch[0], skip_views[si])
-        x, cin = skip_views[si], ch[0]
-        si += 1
-        for i in range(L):
-            cout = ch[i]
-            for j in range(cfg.layers_per_block):
-                rname = f"down_blocks.{i}.resnets.{j}"
-                dst = skip_views[si]
-                if cfg.transformer_layers[i]:
-                    r_out = persist(rows_at(i), cout)
-                    resnet(rname, x, cin, cout, i, r_out)
-                    transformer(f"down_blocks.{i}.attentions.{j}", r_out, cout, i, dst)
-                else:
-                    resnet(rname, x, cin, cout, i, dst)
-                x, cin = dst, cout
-                si += 1
-            if i < L - 1:
-                nm = f"down_blocks.{i}.downsamplers.0.conv"
-                h_, w_ = res_hw[i]
-                cols = scratch("im2col", rows_at(i + 1), 9 * cout)
-                P.im2col_s2(x, B, h_, w_, cout, cols)
-                dst = skip_views[si]
-                P.gemm(cols, Wt[nm + ".w"], cout, 1, 1, rows_at(i + 1), dst, bias=Wt[nm + ".b"])
-                x = dst
-                si += 1
-        # ---- mid ----------------------------------------------------------------------------
-        lv, cm = L - 1, ch[-1]
-        m1 = persist(rows_at(lv), cm)
-        resnet("mid_block.resnets.0", x, cm, cm, lv, m1)
-        m2 = persist(rows_at(lv), cm)
-        transformer("mid_block.attentions.0", m1, cm, lv, m2)
-        resnet("mid_block.resnets.1", m2, cm, cm, lv, cats[0]["hidden"])
+        def down_mid(P, prm, dsts, mid_dst):
+            """The down path and the mid block of a net whose conv_in output is in ``dsts[0]``: each resnet /
+            attention output and each downsampler output goes to the next of ``dsts`` (production order), the mid
+            block's output to ``mid_dst``.  The UNet passes its concat-buffer skip views, a ControlNet its own
+            buffers; ``prm``: that net's packed weights, time-embedding projections and transformer depths."""
+            Wt = prm["W"]
+            x, cin = dsts[0], ch[0]
+            si = 1
+            for i in range(L):
+                cout = ch[i]
+                for j in range(cfg.layers_per_block):
+                    rname = f"down_blocks.{i}.resnets.{j}"
+                    dst = dsts[si]
+                    if prm["depths"][i]:
+                        r_out = persist(rows_at(i), cout)
+                        resnet(P, prm, rname, x, cin, cout, i, r_out)
+                        transformer(P, prm, f"down_blocks.{i}.attentions.{j}", r_out, cout, i, dst)
+                    else:
+                        resnet(P, prm, rname, x, cin, cout, i, dst)
+                    x, cin = dst, cout
+                    si += 1
+                if i < L - 1:
+                    nm = f"down_blocks.{i}.downsamplers.0.conv"
+                    h_, w_ = res_hw[i]
+                    cols = scratch("im2col", rows_at(i + 1), 9 * cout)
+                    P.im2col_s2(x, B, h_, w_, cout, cols)
+                    dst = dsts[si]
+                    P.gemm(cols, Wt[nm + ".w"], cout, 1, 1, rows_at(i + 1), dst, bias=Wt[nm + ".b"])
+                    x = dst
+                    si += 1
+            lv, cm = L - 1, ch[-1]
+            m1 = persist(rows_at(lv), cm)
+            resnet(P, prm, "mid_block.resnets.0", x, cm, cm, lv, m1)
+            m2 = persist(rows_at(lv), cm)
+            transformer(P, prm, "mid_block.attentions.0", m1, cm, lv, m2)
+            resnet(P, prm, "mid_block.resnets.1", m2, cm, cm, lv, mid_dst)
+        self.down_mid = down_mid
+
+        # ---- down path + mid ------------------------------------------------------------------
+        P.conv_in(self.x_in, Wt["conv_in.w"], Wt["conv_in.b"], ch[0], skip_views[0])
+        down_mid(P, unet, skip_views, cats[0]["hidden"])
+        n_down_mid = len(P.ops)          # a ControlNet's records go here, after the UNet's mid block read its input
         # ---- up path ------------------------------------------------------------------------
         ci = 0
         rev_depth = list(reversed(cfg.transformer_layers))
@@ -377,10 +398,10 @@ class _Lowering:
                 rname = f"up_blocks.{i}.resnets.{j}"
                 if rev_depth[i]:
                     r_out = persist(rows_at(lvl), cout)
-                    resnet(rname, cat["buf"], cin_total, cout, lvl, r_out)
-                    transformer(f"up_blocks.{i}.attentions.{j}", r_out, cout, lvl, dst)
+                    resnet(P, unet, rname, cat["buf"], cin_total, cout, lvl, r_out)
+                    transformer(P, unet, f"up_blocks.{i}.attentions.{j}", r_out, cout, lvl, dst)
                 else:
-                    resnet(rname, cat["buf"], cin_total, cout, lvl, dst)
+                    resnet(P, unet, rname, cat["buf"], cin_total, cout, lvl, dst)
                 ci += 1
                 x = dst
             if i < L - 1:
@@ -394,5 +415,30 @@ class _Lowering:
         no = scratch("n1", rows_at(0), ch[0])
         P.groupnorm(x, B, H * W, ch[0], groups, Wt["conv_norm_out.g"], Wt["conv_norm_out.b"], 1e-5, 1, no, self.ws)
         lower_conv_out(P, Wt, no, B, H, W, ch[0], cfg.out_channels, self.eps, scratch)
+        # with a ControlNet: a second step program over the same buffers, the UNet's records with the ControlNet's
+        # between the mid block and the up path
+        self.prog_step_cn = None
+        if net.controlnet is not None:
+            from .controlnet import lower_controlnet
+            PX = Program(net.dev_index)
+            lower_controlnet(self, PX, net.controlnet)
+            self.prog_step_cn = Program(net.dev_index)
+            self.prog_step_cn.ops = P.ops[:n_down_mid] + PX.ops + P.ops[n_down_mid:]
+            self.prog_step_cn.keep = P.keep + PX.keep
+            self.prog_step_cn.finalize()
         P.finalize()
         PC.finalize()
+
+    def embed(self, P, packed, temb_in):
+        """A net's time + added-condition embedding from the sinusoid features ``temb_in`` and ``self.add_in``:
+        returns all its resnets' SiLU(emb) projections [B, packed.temb_total]."""
+        Wt, B, T = packed.w, self.B, packed.cfg.time_embed_dim
+        t1, a1, temb, emb = (self.persist(B, T) for _ in range(4))
+        P.linear_small(temb_in, Wt["time_embedding.linear_1.w"], t1, bias=Wt["time_embedding.linear_1.b"], act_out=1)
+        P.linear_small(t1, Wt["time_embedding.linear_2.w"], temb, bias=Wt["time_embedding.linear_2.b"])
+        P.linear_small(self.add_in, Wt["add_embedding.linear_1.w"], a1, bias=Wt["add_embedding.linear_1.b"],
+                       act_out=1)
+        P.linear_small(a1, Wt["add_embedding.linear_2.w"], emb, bias=Wt["add_embedding.linear_2.b"], addend=temb)
+        temb_all = self.persist(B, packed.temb_total)
+        P.linear_small(emb, Wt["temb_all.w"], temb_all, bias=Wt["temb_all.b"], act_in=1)
+        return temb_all
