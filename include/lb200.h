@@ -27,7 +27,8 @@
  *    variant takes a trailing ``int dtype`` (LB_DTYPE_F16 or LB_DTYPE_BF16, the
  *    element type of its 16-bit tensors; any other value is an error):
  *    lb_groupnorm, lb_conv_in, lb_upsample_nearest, lb_latent_prep,
- *    lb_softmax_rows, lb_postprocess_u8 and lb_nhwc_to_nchw.  A bf16 call keeps
+ *    lb_softmax_rows, lb_postprocess_u8, lb_nhwc_to_nchw, lb_image_conv_in and
+ *    lb_add_noise_rows.  A bf16 call keeps
  *    the fp16 call's layouts, strides, alignment rules and fp32 arithmetic;
  *    only the stored element type differs, except where an entry point says
  *    otherwise.
@@ -294,6 +295,31 @@ int lb_cond_conv(lb_ctx* ctx, const void* x, int64_t ld_x, int B, int H, int W, 
                  const void* w_packed, const void* bias, int Cout, int stride, int silu, void* out, int64_t ldo,
                  void* stream);
 
+/* ---- VAE encoder and img2img start (diffusers 0.25 AutoencoderKL.encode, scheduler.add_noise) ------------------
+ * lb_image_conv_in: the encoder's conv_in on a uint8 image: lb_cond_conv's direct 3x3 pad-1 stride-1 convolution of
+ *   x [B*H*W pixels, ld_x bytes apart, Cin <= 8 channels] into NHWC out [B*H*W, Cout] (row stride ldo), with
+ *   VaeImageProcessor.preprocess fused into the read: every input u becomes r(2 (u / 255) - 1), fp32 arithmetic and
+ *   one rounding r to ``dtype``.  Weights [ky][kx][Cin][Cout] and bias of type ``dtype``, fp32 accumulation,
+ *   y = r(acc + bias).  Cout a multiple of 8.
+ * lb_im2col_s2_pad01: the patch matrix of Downsample2D(padding=0): F.pad(x, (0, 1, 0, 1)) then a 3x3 stride-2 conv
+ *   without padding; like lb_im2col_s2 (out [B*Ho*Wo, 9*C], column (ky*3 + kx)*C + c, then lb_gemm with taps = 1),
+ *   with Ho = floor((H - 2) / 2) + 1 (likewise Wo) and H, W >= 2.  It copies 2-byte elements: fp16 and bf16 alike.
+ * lb_add_noise_rows: out[r] = add_noise(x0, noise, coeffs[r]) for r < rows, fp16 [rows, n] rows n elements apart:
+ *   the forward-diffused rows of a trajectory that starts part-way down the schedule, and its start latent.  coeffs
+ *   (device, fp16 [rows][2]) holds each row's (a, b); with h = fp16 rounding and x = h(x0):
+ *     form 0:  h(x + h(noise * b))              Euler / Euler-ancestral: x0 + noise * sigma
+ *     form 1:  h(h(a * x) + h(b * noise))       LCM, DPM-Solver++: alpha_t * x0 + sigma_t * noise
+ *   (scheduler.add_noise on fp16 CUDA tensors, diffusers 0.25.0).  x0 is fp16 or bf16 (``dtype``), noise fp16.
+ *   nonfinite_count_dev (optional, device int) is incremented by the number of non-finite x0 elements; rows may be 0,
+ *   and then the call only counts.
+ */
+int lb_image_conv_in(lb_ctx* ctx, const void* img_u8, int64_t ld_x, int B, int H, int W, int Cin,
+                     const void* w_packed, const void* bias, int Cout, void* out, int64_t ldo, void* stream,
+                     int dtype);
+int lb_im2col_s2_pad01(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out, void* stream);
+int lb_add_noise_rows(lb_ctx* ctx, const void* x0, const void* noise, const void* coeffs_dev, int form, int64_t n,
+                      int rows, void* out, int* nonfinite_count_dev, void* stream, int dtype);
+
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
  * lb_latent_prep: post_quant_conv(latents / scaling_factor) as a per-pixel CxC fp32 matrix (scale folded in).
  * lb_softmax_rows: row softmax of an fp16 matrix (the VAE mid-block single-head attention, head dim 512,
@@ -360,13 +386,15 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * LB_OP_CONV_IN_ADD (lb_conv_in_add) and LB_OP_COND_CONV (lb_cond_conv) use the ``conv`` member: CONV_IN_ADD reads
  * x, B, Cin, H, W, w, bias, Cout, out, ld_out, addend, ld_add (act must be 0); COND_CONV reads x, ld_x, B, Cin, H, W,
  * w, bias, Cout, out, ld_out, stride, in_u8 and act as lb_cond_conv's ``silu``.
+ * LB_OP_IMAGE_CONV_IN (lb_image_conv_in) uses the ``conv`` member's x, ld_x, B, Cin, H, W, w, bias, Cout, out and
+ * ld_out, with lb_op.dtype; LB_OP_IM2COL_S2_PAD01 (lb_im2col_s2_pad01) uses ``resample`` like LB_OP_IM2COL_S2.
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
     LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
     LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17,
-    LB_OP_CONV_IN_ADD = 19, LB_OP_COND_CONV = 20
+    LB_OP_CONV_IN_ADD = 19, LB_OP_COND_CONV = 20, LB_OP_IMAGE_CONV_IN = 21, LB_OP_IM2COL_S2_PAD01 = 22
 };
 typedef struct lb_op {
     int32_t kind;
@@ -385,7 +413,7 @@ typedef struct lb_op {
         struct { const void* x; int64_t ld_x; int32_t B, Cin, H, W; const void* w; const void* bias;
                  int32_t Cout; void* out; int64_t ld_out; int32_t act; float in_scale;
                  const void* addend; int64_t ld_add; int32_t stride, in_u8; } conv;
-        /* UPSAMPLE_NEAREST: output Ho x Wo (see lb_upsample_nearest); IM2COL_S2: Ho, Wo unused */
+        /* UPSAMPLE_NEAREST: output Ho x Wo (see lb_upsample_nearest); IM2COL_S2 and IM2COL_S2_PAD01: Ho, Wo unused */
         struct { const void* x; int64_t ld_x; int32_t B, H, W, C; void* out; int64_t ld_out; int32_t Ho, Wo; } resample;
         /* LATENT_PREP: x,w,bias,out,B,C,n=h*w; SOFTMAX_ROWS: x,ld_x,out,ld_out,n=rows,C=cols;
          * POSTPROCESS_U8: x,out,B,C,n=h*w, w = optional device int counter of non-finite pixels;

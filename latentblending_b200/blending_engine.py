@@ -59,6 +59,8 @@ class BlendingEngine():
         self.text_embedding2 = None
         self.image1_lowres = None
         self.image2_lowres = None
+        self.init_image1 = None               # image keyframes (set_init_image1/2): dict(image, strength, latents)
+        self.init_image2 = None
         self.negative_prompt = None
         self.set_guidance_scale()
         self.multi_transition_img_first = None
@@ -186,6 +188,60 @@ class BlendingEngine():
 
     def set_image2(self, image):
         self.image2_lowres = image
+
+    def set_init_image1(self, image, strength=0.3):
+        """Start keyframe 1 from ``image`` (a PIL image or an HxWx3 uint8 array) as img2img does: its trajectory is
+        the image's VAE latents forward-diffused with seed1's noise down to the step ``strength`` selects, then
+        denoised under prompt 1.  ``strength`` in (0, 1] has diffusers' img2img meaning (default 0.3, that
+        pipeline's default).  ``None`` returns the keyframe to text-only.  Raises ValueError for a pipe without a
+        KL VAE encoder and for a strength that leaves no step to denoise."""
+        self.init_image1 = self._init_state(image, strength)
+
+    def set_init_image2(self, image, strength=0.3):
+        """set_init_image1 for keyframe 2 (seed2, prompt 2)."""
+        self.init_image2 = self._init_state(image, strength)
+
+    def _init_state(self, image, strength):
+        if image is None:
+            return None
+        from .schedulers import img2img_start
+        img2img_start(self.num_inference_steps, strength)          # the strength's range and step count
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+                raise ValueError(f"an image array must be HxWx3 uint8 (got {image.dtype} {image.shape})")
+            image = Image.fromarray(image)
+        elif not isinstance(image, Image.Image):
+            raise TypeError(f"the image must be a PIL image or an HxWx3 uint8 array (got {type(image)})")
+        st = dict(image=image.convert("RGB"), strength=float(strength), latents={})
+        self._init_latents(st)          # encoded now at the current size: a pipe without an encoder raises here
+        return st
+
+    def _init_latents(self, st):
+        """The keyframe image's latents at the current output size, encoded once per size."""
+        key = (self.dh.height_latent, self.dh.width_latent)
+        if key not in st["latents"]:
+            enc = getattr(self.dh, "image2latent_native", None) or self.dh.image2latent
+            st["latents"][key] = enc(st["image"])
+        return st["latents"][key]
+
+    def _init_start(self, st):
+        """First denoised step of a keyframe: 0 for text, get_timesteps' start index for an image."""
+        if st is None:
+            return 0
+        from .schedulers import img2img_start
+        return img2img_start(self.num_inference_steps, st["strength"])
+
+    def _outer_job(self, which):
+        """(job, start step) of outer trajectory ``which`` (0: keyframe 1, 1: keyframe 2) for run_diffusion_sd_xl_multi."""
+        st = self.init_image1 if which == 0 else self.init_image2
+        seed = self.seed1 if which == 0 else self.seed2
+        job = dict(text_embeddings=self.get_mixed_conditioning(which)[0])
+        if st is None:
+            job["latents_start"] = self.get_noise(seed)
+        else:
+            job["init"] = (self._init_latents(st), self.dh.init_noise(seed))
+        job["noise_fn"] = self._noise_source(float(which))
+        return job, self._init_start(st)
 
     def set_num_inference_steps(self, num_inference_steps=None):
         if num_inference_steps is None:
@@ -434,6 +490,14 @@ class BlendingEngine():
         return self._finish_transition()
 
     def compute_latents1(self, return_image=False):
+        if self.init_image1 is not None:
+            job, i0 = self._outer_job(0)
+            self.dh.set_num_inference_steps(self.num_inference_steps)
+            ev0, ev1 = self._events()
+            list_latents1 = self.dh.run_diffusion_sd_xl_multi([job], idx_start=i0)[0]
+            self._finish_timing(ev0, ev1, steps=self.num_inference_steps - i0)
+            self.tree_latents[0] = list_latents1
+            return self.dh.latent2image(list_latents1[-1]) if return_image else list_latents1
         list_conditionings = self.get_mixed_conditioning(0)
         ev0, ev1 = self._events()
         latents_start = self.get_noise(self.seed1)
@@ -457,22 +521,32 @@ class BlendingEngine():
     def _compute_latents_pair(self):
         """compute_latents1 + compute_latents2 advanced in lockstep through batch-4 UNet forwards (same results:
         the two trajectories are independent, or -- with branch-1 crossfeed -- trajectory 2 reads step i-1 of
-        trajectory 1, which the lockstep loop has already produced)."""
+        trajectory 1, which the lockstep loop has already produced).  Keyframes that start at different steps (an
+        image keyframe, or two with different strengths) run one after the other instead: batch invariance makes the
+        results the same."""
+        if self._init_start(self.init_image1) != self._init_start(self.init_image2):
+            return self.compute_latents1(), self.compute_latents2()
         self.dh.set_num_inference_steps(self.num_inference_steps)
-        job1 = dict(text_embeddings=self.get_mixed_conditioning(0)[0], latents_start=self.get_noise(self.seed1),
-                    noise_fn=self._noise_source(0.0))
-        job2 = dict(text_embeddings=self.get_mixed_conditioning(1)[0], latents_start=self.get_noise(self.seed2),
-                    noise_fn=self._noise_source(1.0))
+        job1, i0 = self._outer_job(0)
+        job2, _ = self._outer_job(1)
         if self.branch1_crossfeed_power > 0.0:
             job2.update(list_latents_mixing=("job", 0), mixing_coeffs=self._branch1_crossfeed_coeffs())
         ev0, ev1 = self._events()
-        list_latents1, list_latents2 = self.dh.run_diffusion_sd_xl_multi([job1, job2], idx_start=0)
-        self._finish_timing(ev0, ev1, branches=2)
+        list_latents1, list_latents2 = self.dh.run_diffusion_sd_xl_multi([job1, job2], idx_start=i0)
+        self._finish_timing(ev0, ev1, branches=2, steps=self.num_inference_steps - i0)
         self.tree_latents[0] = list_latents1
         self.tree_latents[-1] = list_latents2
         return list_latents1, list_latents2
 
     def compute_latents2(self, return_image=False):
+        if self.init_image2 is not None:
+            job, i0 = self._outer_job(1)
+            if self.branch1_crossfeed_power > 0.0:       # applies from the first denoised step on
+                job.update(list_latents_mixing=self.tree_latents[0], mixing_coeffs=self._branch1_crossfeed_coeffs())
+            self.dh.set_num_inference_steps(self.num_inference_steps)
+            list_latents2 = self.dh.run_diffusion_sd_xl_multi([job], idx_start=i0)[0]
+            self.tree_latents[-1] = list_latents2
+            return self.dh.latent2image(list_latents2[-1]) if return_image else list_latents2
         list_conditionings = self.get_mixed_conditioning(1)
         latents_start = self.get_noise(self.seed2)
         if self.branch1_crossfeed_power > 0.0:
@@ -692,6 +766,7 @@ class BlendingEngine():
 
     def swap_forward(self):
         self.tree_latents[0] = self.tree_latents[-1]
+        self.init_image1, self.init_image2 = self.init_image2, None
         self.prompt1 = self.prompt2
         self.text_embedding1 = self.text_embedding2
         self.tree_final_imgs = []
@@ -745,13 +820,15 @@ class BlendingEngine():
             return e0, e1
         return time.time(), None
 
-    def _finish_timing(self, e0, e1, branches=1):
+    def _finish_timing(self, e0, e1, branches=1, steps=None):
+        """``steps``: the denoise steps each branch ran (default all; fewer for an image keyframe)."""
+        steps = self.num_inference_steps if steps is None else steps
         if e1 is None:
-            self.dt_unet_step = (time.time() - e0) / (self.num_inference_steps * branches)
+            self.dt_unet_step = (time.time() - e0) / (steps * branches)
             return
         e1.record()
         # resolved lazily by set_branching / get_time_based_branching: no host sync inside the transition
-        self._pending_timing = (e0, e1, branches, self.num_inference_steps)
+        self._pending_timing = (e0, e1, branches, steps)
 
     def _resolve_timing(self):
         """dt_unet_step tracks the last outer trajectory like blending_engine.py:379-386 (time per UNet step of ONE

@@ -234,12 +234,16 @@ upsample_nearest_kernel(const __half* __restrict__ x, long long ld, int B, int H
     }
 }
 
-// ---- im2col for the 3x3 stride-2 pad-1 downsample convs: out[B*Ho*Wo, 9*C], K order (ky,kx,c) ------
+// ---- im2col for the 3x3 stride-2 downsample convs: out[B*Ho*Wo, 9*C], K order (ky,kx,c) ------
+// kPadLo = 1: zero padding 1 on every side (the UNet's Downsample2D), Ho = floor((H + 2 - 3)/2) + 1.
+// kPadLo = 0: F.pad(x, (0, 1, 0, 1)) then no padding (the VAE encoder's Downsample2D(padding=0)),
+//             Ho = floor((H + 1 - 3)/2) + 1.  The kernel copies 16-byte channel vectors: fp16 and bf16 alike.
+template <int kPadLo>
 __global__ void __launch_bounds__(kThreads)
 im2col_s2_kernel(const __half* __restrict__ x, long long ld, int B, int H, int W, int C, __half* __restrict__ out) {
     pdl_launch_dependents();
     pdl_wait();
-    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;   // floor((H + 2 - 3)/2) + 1
+    const int Ho = kPadLo ? (H + 1) / 2 : (H - 2) / 2 + 1, Wo = kPadLo ? (W + 1) / 2 : (W - 2) / 2 + 1;
     const int vecs = C >> 3;
     const long long total = (long long)B * Ho * Wo * 9 * vecs;
     for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
@@ -247,7 +251,7 @@ im2col_s2_kernel(const __half* __restrict__ x, long long ld, int B, int H, int W
         const int tap = (int)((i / vecs) % 9);
         const long long opix = i / ((long long)vecs * 9);
         const int xo = (int)(opix % Wo), yo = (int)((opix / Wo) % Ho), b = (int)(opix / ((long long)Wo * Ho));
-        const int yy = 2 * yo + tap / 3 - 1, xx = 2 * xo + tap % 3 - 1;
+        const int yy = 2 * yo + tap / 3 - kPadLo, xx = 2 * xo + tap % 3 - kPadLo;
         uint4 val = make_uint4(0, 0, 0, 0);
         if (yy >= 0 && yy < H && xx >= 0 && xx < W)
             val = *reinterpret_cast<const uint4*>(x + (((long long)b * H + yy) * W + xx) * ld + v * 8);
@@ -383,8 +387,21 @@ extern "C" int lb_im2col_s2(lb_ctx* ctx, const void* x, int64_t ld, int B, int H
     LB_REQUIRE(ctx && x && out, "lb_im2col_s2: null argument");
     LB_REQUIRE(C % 8 == 0 && ld % 8 == 0, "lb_im2col_s2: C and stride must be multiples of 8");
     const long long total = (long long)B * ((H + 1) / 2) * ((W + 1) / 2) * 9 * (C / 8);
-    lb_launch_pdl(im2col_s2_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream), (const __half*)x, ld, B, H, W, C,
+    lb_launch_pdl(im2col_s2_kernel<1>, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream), (const __half*)x, ld, B, H, W, C,
                                                                                         (__half*)out);
+    LB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int lb_im2col_s2_pad01(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int W, int C, void* out,
+                                  void* stream) {
+    LB_REQUIRE(ctx && x && out, "lb_im2col_s2_pad01: null argument");
+    LB_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ld >= C && lb_aligned16(x) && lb_aligned16(out),
+               "lb_im2col_s2_pad01: C and stride must be multiples of 8, bases 16-byte aligned");
+    LB_REQUIRE(B >= 1 && H >= 2 && W >= 2, "lb_im2col_s2_pad01: needs H, W >= 2 (got B %d H %d W %d)", B, H, W);
+    const long long total = (long long)B * ((H - 2) / 2 + 1) * ((W - 2) / 2 + 1) * 9 * (C / 8);
+    lb_launch_pdl(im2col_s2_kernel<0>, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream),
+                  (const __half*)x, ld, B, H, W, C, (__half*)out);
     LB_LAUNCH_CHECK();
     return 0;
 }

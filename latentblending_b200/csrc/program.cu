@@ -52,7 +52,7 @@ struct lb_program {
 static bool kind_has_dtype(int kind) {
     switch (kind) {
         case LB_OP_GROUPNORM: case LB_OP_LATENT_PREP: case LB_OP_CONV_IN: case LB_OP_UPSAMPLE_NEAREST:
-        case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS:
+        case LB_OP_NHWC_TO_NCHW: case LB_OP_POSTPROCESS_U8: case LB_OP_SOFTMAX_ROWS: case LB_OP_IMAGE_CONV_IN:
             return true;
         default:
             return false;
@@ -96,6 +96,7 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_UPSAMPLE_NEAREST: case LB_OP_IM2COL_S2: case LB_OP_GROUPNORM: case LB_OP_LAYERNORM:
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
+            case LB_OP_IMAGE_CONV_IN: case LB_OP_IM2COL_S2_PAD01:
                 break;
             case LB_OP_CONV_IN_ADD: case LB_OP_COND_CONV:
                 if (ops[i].kind == LB_OP_CONV_IN_ADD && ops[i].u.conv.act != 0) {
@@ -243,6 +244,12 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
                                  a.out, a.ld_out, stream);
                 break;
             }
+            case LB_OP_IMAGE_CONV_IN: {
+                const auto& a = o.u.conv;
+                e = lb_image_conv_in(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.Cin, a.w, a.bias, a.Cout, a.out, a.ld_out,
+                                     stream, o.dtype);
+                break;
+            }
             case LB_OP_UPSAMPLE_NEAREST: {
                 const auto& a = o.u.resample;
                 e = lb_upsample_nearest(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, a.ld_out, a.Ho, a.Wo, stream,
@@ -252,6 +259,11 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             case LB_OP_IM2COL_S2: {
                 const auto& a = o.u.resample;
                 e = lb_im2col_s2(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, stream);
+                break;
+            }
+            case LB_OP_IM2COL_S2_PAD01: {
+                const auto& a = o.u.resample;
+                e = lb_im2col_s2_pad01(ctx, a.x, a.ld_x, a.B, a.H, a.W, a.C, a.out, stream);
                 break;
             }
             case LB_OP_GROUPNORM: {

@@ -12,6 +12,10 @@
 // values in registers but apply the same roundings, so results are bit-identical
 // to the op-by-op oracle (oracle/schedulers.py, oracle/holder.py).
 // HBM-bound: (2B+1) reads + 2 writes of n fp16 elements.
+//
+// add_noise_rows_kernel starts a trajectory part-way down the schedule from an image's latents (img2img): every
+// forward-diffused row the denoise loop skips, plus its start latent, in one launch (scheduler.add_noise of diffusers
+// 0.25.0 on fp16 CUDA tensors, with the same fp16 roundings).
 #include "common.cuh"
 
 namespace {
@@ -273,4 +277,58 @@ extern "C" int lb_cfg_dpm_step(lb_ctx* ctx, const void* latents, const void* eps
     const float s[kStepScalars] = {sigma_s, inv_alpha_s, inv_r0, c_x, c_0, c_1, c_n};
     return launch_cfg_step<DpmUpdate>("lb_cfg_dpm_step", ctx, latents, eps, eps_text, noise, out, traj, n, use_cfg,
                                       guidance, s, scaled_next, scaled_batch, next_divisor, stream, x0_prev, x0_out);
+}
+
+namespace {
+
+// out[r] = add_noise(x0, eps, coeffs[r]), every op rounded to fp16 like the reference's fp16 tensors (h = rounding):
+//   form 0 (Euler, Euler-ancestral):  h(x + h(eps * b))             x0 + noise * sigma
+//   form 1 (LCM, DPM-Solver++):       h(h(a * x) + h(b * eps))      sqrt_alpha * x0 + sqrt_one_minus_alpha * noise
+// x = h(x0): a bf16 x0 is rounded to fp16 first (the pipeline's .to(fp16)).  Each thread reads x0 and eps once and
+// writes every row.  `nonfinite` (optional) counts the non-finite x0 elements.
+template <typename TX>
+__global__ void __launch_bounds__(kThreads)
+add_noise_rows_kernel(const TX* __restrict__ x0, const __half* __restrict__ eps, const __half* __restrict__ coeffs,
+                      int form, long long n, int rows, __half* __restrict__ out, int* __restrict__ nonfinite) {
+    pdl_launch_dependents();
+    pdl_wait();
+    int bad = 0;
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
+        const float xr = LbType<TX>::to_f(x0[i]);
+        bad += !isfinite(xr);
+        const float x = h(xr);
+        const float e = __half2float(eps[i]);
+        for (int r = 0; r < rows; ++r) {
+            const float a = __half2float(coeffs[2 * r]), b = __half2float(coeffs[2 * r + 1]);
+            const float v = form == 0 ? h(x + h(e * b)) : h(h(a * x) + h(b * e));
+            out[(long long)r * n + i] = __float2half_rn(v);
+        }
+    }
+    if (nonfinite != nullptr && __any_sync(0xffffffffu, bad != 0)) {
+        bad = __reduce_add_sync(0xffffffffu, bad);
+        if ((threadIdx.x & 31) == 0) atomicAdd(nonfinite, bad);
+    }
+}
+
+}  // namespace
+
+extern "C" int lb_add_noise_rows(lb_ctx* ctx, const void* x0, const void* noise, const void* coeffs_dev, int form,
+                                 int64_t n, int rows, void* out, int* nonfinite_count_dev, void* stream, int dtype) {
+    LB_REQUIRE(dtype == LB_DTYPE_F16 || dtype == LB_DTYPE_BF16, "lb_add_noise_rows: unknown dtype %d", dtype);
+    LB_REQUIRE(ctx && x0 && noise, "lb_add_noise_rows: null argument");
+    LB_REQUIRE(form == 0 || form == 1, "lb_add_noise_rows: unknown form %d (0 = x0 + b*noise, 1 = a*x0 + b*noise)", form);
+    LB_REQUIRE(n > 0 && rows >= 0, "lb_add_noise_rows: bad sizes n %lld rows %d", (long long)n, rows);
+    LB_REQUIRE(rows == 0 || (coeffs_dev && out), "lb_add_noise_rows: rows > 0 needs coeffs and out");
+    unsigned grid = (unsigned)lb_ceil_div(n, (int64_t)kThreads);
+    if (grid > (unsigned)ctx->sm_count * 8) grid = (unsigned)ctx->sm_count * 8;
+    if (dtype == LB_DTYPE_BF16)
+        lb_launch_pdl(add_noise_rows_kernel<__nv_bfloat16>, grid, kThreads, 0, lb_stream(stream),
+                      (const __nv_bfloat16*)x0, (const __half*)noise, (const __half*)coeffs_dev, form, (long long)n,
+                      rows, (__half*)out, nonfinite_count_dev);
+    else
+        lb_launch_pdl(add_noise_rows_kernel<__half>, grid, kThreads, 0, lb_stream(stream), (const __half*)x0,
+                      (const __half*)noise, (const __half*)coeffs_dev, form, (long long)n, rows, (__half*)out,
+                      nonfinite_count_dev);
+    LB_LAUNCH_CHECK();
+    return 0;
 }

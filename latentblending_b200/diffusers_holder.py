@@ -56,6 +56,7 @@ class DiffusersHolder:
                                              getattr(pipe, "controlnet_cond_channels", None) or COND_CHANNELS)
         self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device, controlnet=self.controlnet)
         self.vae = None
+        self.vae_encoder = None       # built on the first image2latent, in the decoder's storage type
         self.set_vae_dtype(getattr(pipe, "vae_dtype", "fp16"))
         self.noise_fn = None          # tests: inject the ancestral-step noise, noise_fn(i, shape)
         self.noise_fn_multi = None    # same for run_diffusion_sd_xl_multi with k > 1: noise_fn_multi(job, i, shape)
@@ -90,6 +91,8 @@ class DiffusersHolder:
             self.vae = VAEDecoderB200(p.vae_state_dict, p.vae_channels, p.vae_scaling_factor, self.device,
                                       dtype=VAE_DTYPES[vae_dtype])
         self.vae_dtype = vae_dtype
+        if self.vae_encoder is not None and self.vae_encoder.dtype != VAE_DTYPES[vae_dtype]:
+            self.vae_encoder = None
 
     def set_num_inference_steps(self, num_inference_steps):
         self.num_inference_steps = num_inference_steps
@@ -174,10 +177,78 @@ class DiffusersHolder:
 
     def get_noise(self, seed=420):
         """randn([1,4,h,w], fp16, CUDA generator(seed)) * init_noise_sigma -- as pipe.prepare_latents does."""
+        return self.init_noise(seed) * self.pipe.scheduler.init_noise_sigma.to(device=self.device, dtype=torch.float16)
+
+    def init_noise(self, seed=420):
+        """randn([1,4,h,w], fp16, CUDA generator(seed)): get_noise's draw before ``* init_noise_sigma``, the noise an
+        img2img keyframe is forward-diffused with (a seed gives the same noise field for a text or an image keyframe)."""
         g = torch.Generator(device=self.device).manual_seed(int(seed))
-        lat = torch.randn((1, self.pipe.unet_cfg.in_channels, self.height_latent, self.width_latent), generator=g,
-                          device=self.device, dtype=torch.float16)
-        return lat * self.pipe.scheduler.init_noise_sigma.to(device=self.device, dtype=torch.float16)
+        return torch.randn((1, self.pipe.unet_cfg.in_channels, self.height_latent, self.width_latent), generator=g,
+                           device=self.device, dtype=torch.float16)
+
+    # ---- image keyframes (img2img) ----------------------------------------------------------------------------
+    def _encoder(self):
+        """The native KL VAE encoder in the decoder's storage type; ValueError when the pipe has none."""
+        if self.vae_encoder is None:
+            p = self.pipe
+            if getattr(p, "vae_kind", "kl") == "tiny":
+                raise ValueError("image keyframes need the KL VAE's encoder; the tiny autoencoder (AutoencoderTiny) "
+                                 "has no native encoder here: load the pipeline with its AutoencoderKL")
+            sd = getattr(p, "vae_encoder_state_dict", None)
+            if sd is None:
+                raise ValueError("image keyframes need the VAE's encoder weights: the pipe's VAE state dict has no "
+                                 "encoder.* / quant_conv.* parameters")
+            from .pipe import VAE_DTYPES
+            from .vae import VAEEncoderB200
+            self.vae_encoder = VAEEncoderB200(sd, p.vae_channels, p.vae_scaling_factor, self.device,
+                                              dtype=VAE_DTYPES[self.vae_dtype])
+        return self.vae_encoder
+
+    def _image_u8(self, image):
+        """A PIL image or HxWx3 uint8 array -> RGB, LANCZOS-resized to the output size (VaeImageProcessor.resize),
+        as a uint8 [H, W, 3] device tensor."""
+        from PIL import Image
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+                raise ValueError(f"an image array must be HxWx3 uint8 (got {image.dtype} {image.shape})")
+            image = Image.fromarray(image)
+        elif not isinstance(image, Image.Image):
+            raise TypeError(f"the image must be a PIL image or an HxWx3 uint8 array (got {type(image)})")
+        image = image.convert("RGB")
+        if image.size != (self.width_img, self.height_img):
+            image = image.resize((self.width_img, self.height_img), resample=Image.LANCZOS)
+        return torch.from_numpy(np.ascontiguousarray(np.array(image))).to(self.device)
+
+    @torch.no_grad()
+    def image2latent_native(self, image):
+        """The image's latents in the encoder's storage type (fp16 or bf16) [1,4,h,w]: scaling_factor times the
+        posterior mean (retrieve_latents(..., sample_mode="argmax")).  Raises when they are not finite."""
+        enc = self._encoder()
+        x0 = enc.encode(self._image_u8(image)).clone()
+        enc.check_finite(x0)
+        return x0
+
+    @torch.no_grad()
+    def image2latent(self, image):
+        """The inverse of latent2image: a PIL image or HxWx3 uint8 array -> [1,4,h,w] fp16 latents at the current
+        output size (scaling_factor times the VAE posterior's mean; a bf16 encode is rounded to fp16)."""
+        return self.image2latent_native(image).to(torch.float16)
+
+    def _write_init_rows(self, init, idx_start, traj, C, h, w):
+        """Rows 0 .. idx_start-1 of ``traj``: the image latents forward-diffused to timesteps[i+1] (one
+        lb_add_noise_rows launch); returns the start latent, add_noise(x0, eps, timesteps[idx_start])."""
+        x0, eps = init
+        if tuple(x0.shape) != (1, C, h, w) or tuple(eps.shape) != (1, C, h, w):
+            raise ValueError(f"init latents / noise {tuple(x0.shape)} / {tuple(eps.shape)} do not match "
+                             f"{(1, C, h, w)}")
+        sched = self.pipe.scheduler
+        idx = list(range(1, idx_start + 1)) if idx_start > 0 else [0]
+        cf = [sched.add_noise_coeffs(i) for i in idx]
+        form = cf[0][0]
+        coeffs = torch.tensor([[a, b] for _, a, b in cf], dtype=torch.float16).to(self.device, non_blocking=True)
+        out = traj[:idx_start] if idx_start > 0 else torch.empty((1, C, h, w), dtype=torch.float16, device=self.device)
+        ops.add_noise_rows(x0.contiguous(), eps.to(torch.float16).contiguous(), coeffs, form, out=out)
+        return out[idx_start - 1:idx_start] if idx_start > 0 else out
 
     @torch.no_grad()
     def decode_to_device(self, latents):
@@ -236,6 +307,9 @@ class DiffusersHolder:
         is exactly run_diffusion_sd_xl's: every kernel on the path is batch-invariant (tests/test_engine_gpu.py).
 
         jobs: dicts with text_embeddings (4-tuple), latents_start, list_latents_mixing, mixing_coeffs and optionally
+        init = (x0, eps) (an image keyframe: rows i < idx_start of the trajectory become x0 forward-diffused to
+        timesteps[i+1] with noise eps, the start latent is add_noise(x0, eps, timesteps[idx_start]), and latents_start
+        is not read; see _write_init_rows),
         guidance_scale (default: self.guidance_scale) and noise_fn(step, shape) (this job's scheduler noise source).  ``list_latents_mixing`` may be ``("job", j)``: mix against
         the trajectory job j is producing in this very call (branch-1 crossfeed reads step i-1, which job j has
         already written).  Returns one len-N list per job (None for i < idx_start, else [1,4,h,w] fp16 views of that
@@ -251,7 +325,8 @@ class DiffusersHolder:
         split = self.cfg_split if cfg_on else None           # without CFG there is nothing to split
         Bj = 1 if (split is not None or not cfg_on) else 2      # UNet batch rows per job ON THIS RANK
         k = len(jobs)
-        _, C, h, w = jobs[0]["latents_start"].shape
+        j0 = jobs[0]
+        _, C, h, w = (j0["init"][0] if j0.get("init") is not None else j0["latents_start"]).shape
         ctxs, texts = [], []
         for job in jobs:
             pe, ne, pp, npool = job["text_embeddings"]
@@ -298,6 +373,12 @@ class DiffusersHolder:
         n = C * h * w
         outs = [[None] * N for _ in jobs]
         trajs = [torch.empty((N, C, h, w), dtype=torch.float16, device=self.device) for _ in jobs]
+        starts = [None] * k
+        for j, job in enumerate(jobs):
+            if job.get("init") is not None:            # an image keyframe: its prefix rows and start latent
+                starts[j] = self._write_init_rows(job["init"], idx_start, trajs[j], C, h, w)
+                for i in range(idx_start):
+                    outs[j][i] = trajs[j][i:i + 1]
         coeffs, mixing, guidance, latents = [], [], [], []
         for job in jobs:
             m = job.get("list_latents_mixing")
@@ -330,7 +411,7 @@ class DiffusersHolder:
             sc = sched.step_scalars[i]
             for j, job in enumerate(jobs):
                 if i == idx_start:
-                    latents[j] = job["latents_start"].clone().contiguous()
+                    latents[j] = (starts[j] if starts[j] is not None else job["latents_start"]).clone().contiguous()
                 if i > 0 and coeffs[j][i] > 0:
                     latents[j] = ops.slerp_rows(latents[j].view(1, n), mixing[j][i - 1].reshape(1, n),
                                                 float(coeffs[j][i])).view(1, C, h, w)

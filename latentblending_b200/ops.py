@@ -323,6 +323,47 @@ def im2col_s2(x, B, H, W, C, out=None):
     return out
 
 
+def im2col_s2_pad01(x, B, H, W, C, out=None):
+    """Patch matrix of Downsample2D(padding=0) (F.pad(x, (0, 1, 0, 1)), 3x3 stride 2) of NHWC fp16 / bf16 rows."""
+    dev = _dev(x)
+    Ho, Wo = (H - 2) // 2 + 1, (W - 2) // 2 + 1
+    if out is None:
+        out = torch.empty((B * Ho * Wo, 9 * C), dtype=x.dtype, device=x.device)
+    _run1(dev, lambda P: P.im2col_s2_pad01(x, B, H, W, C, out))
+    return out
+
+
+def image_conv_in(img_u8, w_packed, bias, Cout, out=None):
+    """The VAE encoder's conv_in of a uint8 HxWx3 image with the preprocess fused (lb_image_conv_in): NHWC
+    [H*W, Cout] of ``w_packed``'s type (fp16 / bf16)."""
+    dev = _dev(img_u8)
+    H, W, _ = img_u8.shape
+    if out is None:
+        out = torch.empty((H * W, Cout), dtype=w_packed.dtype, device=img_u8.device)
+    _run1(dev, lambda P: P.image_conv_in(img_u8.reshape(H * W, -1), 1, H, W, w_packed, bias, Cout, out))
+    return out
+
+
+def add_noise_rows(x0, noise, coeffs, form, out=None, nonfinite=None):
+    """out[r] = add_noise(x0, noise, coeffs[r]) (lb_add_noise_rows): ``x0`` fp16 / bf16 and ``noise`` fp16 with n
+    elements each, ``coeffs`` a device fp16 [rows, 2] of (a, b), ``form`` _cabi.ADD_NOISE_SIGMA (x0 + b*noise) or
+    ADD_NOISE_ALPHA_SIGMA (a*x0 + b*noise); -> fp16 [rows, n].  ``nonfinite`` (device int32[1]) counts non-finite x0
+    elements."""
+    dev = _dev(x0)
+    assert x0.is_contiguous() and noise.is_contiguous() and noise.dtype == torch.float16
+    assert x0.numel() == noise.numel() and coeffs.dtype == torch.float16 and coeffs.is_contiguous()
+    n, rows = x0.numel(), coeffs.shape[0]
+    if out is None:
+        out = torch.empty((rows, n), dtype=torch.float16, device=x0.device)
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.numel() == rows * n
+    from .program import dtype16
+    check(_cabi.load().lb_add_noise_rows(ctx(dev), ptr(x0), ptr(noise), ptr(coeffs), int(form), n, rows, ptr(out),
+                                         ptr(nonfinite), stream_ptr(), dtype16(x0, "add_noise x0")),
+          "lb_add_noise_rows")
+    LAUNCHES[0] += 1
+    return out
+
+
 # ---- VAE-decoder helpers (fp16 or bf16) ---------------------------------------------------------------------------
 
 

@@ -207,6 +207,53 @@ def vae_param_shapes(channels=VAE_CHANNELS, latent=4):
     return P
 
 
+def vae_encoder_param_shapes(channels=VAE_CHANNELS, latent=4, layers_per_block=2):
+    """diffusers state_dict names of an AutoencoderKL's encoder (``encoder.`` stripped) and its ``quant_conv`` ->
+    shapes: conv_in 3 -> C0, down blocks of ``layers_per_block`` resnets (a Downsample2D after all but the last), the
+    mid block, conv_norm_out and conv_out to the 2 * latent moments."""
+    P = OrderedDict()
+
+    def conv(n, i, o, k):
+        P[n + ".weight"] = (o, i, k, k)
+        P[n + ".bias"] = (o,)
+
+    def norm(n, c):
+        P[n + ".weight"] = (c,)
+        P[n + ".bias"] = (c,)
+
+    def resnet(n, i, o):
+        norm(n + ".norm1", i)
+        conv(n + ".conv1", i, o, 3)
+        norm(n + ".norm2", o)
+        conv(n + ".conv2", o, o, 3)
+        if i != o:
+            conv(n + ".conv_shortcut", i, o, 1)
+
+    ch = list(channels)
+    conv("conv_in", 3, ch[0], 3)
+    cout = ch[0]
+    for i, c in enumerate(ch):
+        cin, cout = cout, c
+        for j in range(layers_per_block):
+            resnet(f"down_blocks.{i}.resnets.{j}", cin if j == 0 else cout, cout)
+        if i < len(ch) - 1:
+            conv(f"down_blocks.{i}.downsamplers.0.conv", cout, cout, 3)
+    resnet("mid_block.resnets.0", ch[-1], ch[-1])
+    norm("mid_block.attentions.0.group_norm", ch[-1])
+    for n in ("to_q", "to_k", "to_v", "to_out.0"):
+        P[f"mid_block.attentions.0.{n}.weight"] = (ch[-1], ch[-1])
+        P[f"mid_block.attentions.0.{n}.bias"] = (ch[-1],)
+    resnet("mid_block.resnets.1", ch[-1], ch[-1])
+    norm("conv_norm_out", ch[-1])
+    conv("conv_out", ch[-1], 2 * latent, 3)
+    conv("quant_conv", 2 * latent, 2 * latent, 1)
+    return P
+
+
+# SyntheticSDXLPipe seeds its VAE encoder weights with seed + this offset: no other synthetic state dict uses it
+VAE_ENCODER_SEED_OFFSET = 4099
+
+
 def tiny_vae_param_shapes(config=None):
     """diffusers state_dict names (``decoder.`` stripped) -> shapes of an AutoencoderTiny decoder."""
     from .taesd import decoder_layout, tiny_config
@@ -304,7 +351,7 @@ class SyntheticSDXLPipe:
     def __init__(self, name="stabilityai/stable-diffusion-xl-base-1.0", device="cuda:0", unet_cfg: UNetConfig = None,
                  seed=0, unet_state_dict=None, vae_state_dict=None, vae_channels=VAE_CHANNELS,
                  lpips_state_dict=None, vae_dtype="fp16", vae="kl", scheduler=None, controlnet=None,
-                 controlnet_state_dict=None):
+                 controlnet_state_dict=None, vae_encoder_state_dict=None):
         """``scheduler``: None (Euler for SDXL base, Euler-ancestral for a name with "turbo"), "euler",
         "euler_ancestral", "lcm" (LCMScheduler tables: LCM-LoRA-style with the base UNet, LCM-SDXL-style with
         ``unet_cfg.time_cond_proj_dim`` set) or one of DPM_SCHEDULERS (DPMSolverMultistepScheduler tables for the SDXL
@@ -314,7 +361,9 @@ class SyntheticSDXLPipe:
         default config, scaling_factor 1.0, fp16 only; ``vae_state_dict`` then holds its ``decoder.``-stripped
         weights, seeded by ``random_tiny_vae_state_dict`` when omitted).
         ``controlnet``: None, "full" or "small" (``controlnet_config``): an SDXL ControlNet with seeded weights
-        (``random_controlnet_state_dict``) unless ``controlnet_state_dict`` is given."""
+        (``random_controlnet_state_dict``) unless ``controlnet_state_dict`` is given.
+        ``vae_encoder_state_dict``: the KL VAE's encoder + quant_conv weights (``vae_encoder_param_shapes``), seeded
+        with ``seed + VAE_ENCODER_SEED_OFFSET`` when omitted; a tiny-VAE pipe has no encoder."""
         if vae_dtype not in VAE_DTYPES:
             raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
         if vae not in ("kl", "tiny"):
@@ -351,6 +400,12 @@ class SyntheticSDXLPipe:
             self.vae_state_dict = vae_state_dict if vae_state_dict is not None else \
                 random_state_dict(vae_param_shapes(vae_channels), seed + 1, self.device, damp=0.3)
             self.vae_scaling_factor = 0.13025
+        # the KL encoder (image keyframes, DiffusersHolder.image2latent); the tiny autoencoder has none here
+        self.vae_encoder_state_dict = None
+        if vae == "kl":
+            self.vae_encoder_state_dict = vae_encoder_state_dict if vae_encoder_state_dict is not None else \
+                random_state_dict(vae_encoder_param_shapes(vae_channels), seed + VAE_ENCODER_SEED_OFFSET,
+                                  self.device, damp=0.3)
         self.vae_dtype = vae_dtype
         self.lpips_state_dict = lpips_state_dict
         self.h2d_bytes = 0        # bytes of conditioning copied host->device (bench e2e)
@@ -458,6 +513,7 @@ class DiffusersSDXLPipe:
             # the tiny autoencoder (e.g. madebyollin/taesdxl): its decoder only; fp16, the one precision it has here
             from .taesd import check_config, check_state_dict
             self.vae_kind = "tiny"
+            self.vae_encoder_state_dict = None
             self.vae_config = check_config(vcfg)
             self.vae_state_dict = OrderedDict((k[len("decoder."):], v) for k, v in vsd.items()
                                               if k.startswith("decoder."))
@@ -469,6 +525,10 @@ class DiffusersSDXLPipe:
             self.vae_kind = "kl"
             self.vae_state_dict = OrderedDict((k[len("decoder."):] if k.startswith("decoder.") else k, v)
                                               for k, v in vsd.items() if k.startswith(("decoder.", "post_quant_conv.")))
+            # the encoder of image keyframes (None when the VAE was loaded without one)
+            enc = OrderedDict((k[len("encoder."):] if k.startswith("encoder.") else k, v)
+                              for k, v in vsd.items() if k.startswith(("encoder.", "quant_conv.")))
+            self.vae_encoder_state_dict = enc if any(k.startswith("conv_in.") for k in enc) else None
             self.vae_channels = tuple(vcfg["block_out_channels"] if "block_out_channels" in vcfg
                                       else vcfg.block_out_channels)
             self.vae_scaling_factor = float(vcfg["scaling_factor"] if "scaling_factor" in vcfg else vcfg.scaling_factor)

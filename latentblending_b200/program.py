@@ -8,7 +8,7 @@ import torch
 
 from . import _cabi
 from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_COND_CONV, OP_CONV_IN, OP_CONV_IN_ADD,
-                    OP_EMBED_INPUTS, OP_GEMM,
+                    OP_EMBED_INPUTS, OP_GEMM, OP_IMAGE_CONV_IN, OP_IM2COL_S2_PAD01,
                     OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
                     OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS,
                     OP_UPSAMPLE_NEAREST, Op, check, ctx, stream_ptr)
@@ -197,6 +197,18 @@ class Program:
         d.act, d.stride, d.in_u8 = int(silu), stride, int(x.dtype == torch.uint8)
         self.hold(x, w, bias, out)
 
+    def image_conv_in(self, img_u8, B, H, W, w, bias, Cout, out):
+        """The VAE encoder's conv_in on a uint8 image [B*H*W, >=3] with VaeImageProcessor.preprocess fused
+        (lb_image_conv_in): fp16 or bf16 ``w`` [ky][kx][Cin][Cout], ``bias`` and NHWC ``out`` [B*H*W, >=Cout]."""
+        if img_u8.dtype != torch.uint8:
+            raise _cabi.LB200Error(f"image_conv_in: the image must be uint8 (got {img_u8.dtype})")
+        dt = dtype16(out, "image_conv_in out")
+        _same_dtype(out.dtype, "image_conv_in w / bias / out", w, bias)
+        d = self._new(OP_IMAGE_CONV_IN, dt).u.conv
+        d.x, d.ld_x, d.B, d.Cin, d.H, d.W = _p(img_u8), img_u8.stride(-2), B, img_u8.shape[-1], H, W
+        d.w, d.bias, d.Cout, d.out, d.ld_out = _p(w), _p(bias), Cout, _p(out), out.stride(0)
+        self.hold(img_u8, w, bias, out)
+
     def conv_out_gemm(self, x, B, H, W, Cin, w8, bias8, Cout, out_nchw, tmp):
         """The C0 -> Cout (<= 8) 3x3 output convolution on the tensor-core GEMM: N = 8 (zero-padded weight rows),
         then the Cout live columns go back to NCHW.  ``tmp``: [B*H*W, 8] scratch of the output's type."""
@@ -223,6 +235,15 @@ class Program:
 
     def im2col_s2(self, x, B, H, W, C, out):
         d = self._new(OP_IM2COL_S2).u.resample
+        d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
+        self.hold(x, out)
+
+    def im2col_s2_pad01(self, x, B, H, W, C, out):
+        """Patch matrix [B*Ho*Wo, 9*C] of Downsample2D(padding=0): F.pad(x, (0, 1, 0, 1)), then 3x3 stride 2
+        (lb_im2col_s2_pad01); Ho = (H - 2) // 2 + 1.  fp16 or bf16."""
+        dtype16(x, "im2col_s2_pad01 x")
+        _same_dtype(x.dtype, "im2col_s2_pad01 x / out", out)
+        d = self._new(OP_IM2COL_S2_PAD01).u.resample
         d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
         self.hold(x, out)
 

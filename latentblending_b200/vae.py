@@ -11,12 +11,15 @@ The mid-block single-head attention (head dim 512, S = h*w) is three GEMMs aroun
 scores = (Wq x)(Wk x)^T (1/sqrt(C) folded into Wq), P = softmax_rows(scores), out = P V with V^T
 produced directly by a GEMM with swapped operands; the value bias is folded into the output bias
 (softmax rows sum to one).  Weights use the diffusers state_dict names.
+``VAEEncoderB200`` is the matching encoder (image keyframes, DiffusersHolder.image2latent): the same resnet and
+attention lowering, a fused image-preprocessing conv_in and the asymmetric-pad stride-2 downsamples.
 """
 import torch
 
 from . import _cabi
 from ._cabi import ctx
-from .lowering import Scratch, lower_conv_out, lower_resnet, pack3, pack_resnet
+from .lowering import (Scratch, lower_conv_out, lower_resnet, lower_vae_attention, pack3, pack_resnet,
+                       pack_vae_attention)
 from .program import Program, pack_conv_out8
 
 
@@ -94,15 +97,7 @@ class VAEDecoderB200(DecoderBase):
         self.resnets = [k[: -len(".norm1.weight")] for k in sd if k.endswith(".norm1.weight")]
         for r in self.resnets:
             pack_resnet(W, r, sd, g)
-        a = "mid_block.attentions.0"
-        Cm = sd[a + ".to_q.weight"].shape[0]
-        scale = Cm ** -0.5
-        W["attn.norm.g"], W["attn.norm.b"] = g(a + ".group_norm.weight"), g(a + ".group_norm.bias")
-        W["attn.qk.w"] = torch.cat([(gf(a + ".to_q.weight") * scale), gf(a + ".to_k.weight")], 0).to(dtype).contiguous()
-        W["attn.qk.b"] = torch.cat([(gf(a + ".to_q.bias") * scale), gf(a + ".to_k.bias")], 0).to(dtype).contiguous()
-        W["attn.v.w"] = g(a + ".to_v.weight")
-        W["attn.out.w"] = g(a + ".to_out.0.weight")
-        W["attn.out.b"] = (gf(a + ".to_out.0.bias") + gf(a + ".to_out.0.weight") @ gf(a + ".to_v.bias")).to(dtype).contiguous()
+        pack_vae_attention(W, "mid_block.attentions.0", sd, g, gf, dtype)
         for k in sd:
             if k.endswith("upsamplers.0.conv.weight"):
                 nm = k[: -len(".weight")]
@@ -148,30 +143,8 @@ class _VAELowering:
         P.conv_in(z, Wt["conv_in.w"], Wt["conv_in.b"], C0, x)
         x2 = torch.empty(S, C0, **act)
         resnet("mid_block.resnets.0", x, C0, C0, h, w, x2)
-        # mid-block attention (single head, dim C0)
-        # V^T and the scores take the keys as the GEMM's N, which must be a multiple of 8: hn and qk get S8 >= S rows,
-        # the extra ones zero (never written), so the extra V^T and score columns are exact zeros
-        S8 = -(-S // 8) * 8
-        hn = torch.zeros(S8, C0, **act)
-        P.groupnorm(x2, B, S, C0, groups, Wt["attn.norm.g"], Wt["attn.norm.b"], 1e-6, 0, hn, self.ws)
-        qk = torch.zeros(S8, 2 * C0, **act)
-        P.gemm(hn, Wt["attn.qk.w"], 2 * C0, 1, 1, S, qk, bias=Wt["attn.qk.b"])
-        # P V contracts over the S keys, and the GEMM's K must be a multiple of 64: P and V^T get Sp >= S8 columns, the
-        # extra ones zero, which adds exact zeros to every dot product
-        Sp = -(-S // 64) * 64
-        vT = torch.zeros(C0, Sp, **act)
-        P.gemm(Wt["attn.v.w"], hn, S8, 1, 1, C0, vT[:, :S8], static_w=False)             # V^T = Wv hn^T
-        scores = torch.zeros(S, Sp, **f16)
-        # bf16: the scores are stored in fp16 (LB_GEMM_OUT_F16), whose rounding is 8x finer than bf16's -- the error of
-        # a score s becomes an exp(s) error -- and whose range their modest magnitudes do not approach; the softmax
-        # writes the bf16 P over them (same 2-byte slots), which P V reads as a bf16 operand
-        P.gemm(qk[:, :C0], qk[:, C0:], S8, 1, 1, S, scores[:, :S8], static_w=False)      # (scaled q) k^T
-        probs = scores.view(vae.dtype)
-        P.softmax_rows(scores[:, :S], probs[:, :S])
-        att = sc("h1", S, C0)
-        P.gemm(probs, vT, C0, 1, 1, S, att, static_w=False)                               # P V
         x3 = torch.empty(S, C0, **act)
-        P.gemm(att, Wt["attn.out.w"], C0, 1, 1, S, x3, bias=Wt["attn.out.b"], res=x2)
+        lower_vae_attention(P, Wt, x2, S, C0, groups, self.ws, sc, x3)      # mid-block attention (single head, dim C0)
         x4 = torch.empty(S, C0, **act)
         resnet("mid_block.resnets.1", x3, C0, C0, h, w, x4)
         x, cin, hh, ww = x4, C0, h, w
@@ -194,4 +167,137 @@ class _VAELowering:
         img = torch.empty(1, 3, hh, ww, **act)
         lower_conv_out(P, Wt, no, B, hh, ww, cin, 3, img, sc)
         P.postprocess_u8(img, self.frame, vae.nonfinite)
+        P.finalize()
+
+
+class VAEEncoderB200:
+    """AutoencoderKL encoder (diffusers 0.25.0 ``Encoder`` + ``quant_conv``) on liblb200: a uint8 image in, the
+    posterior mean times ``scaling_factor`` out -- ``retrieve_latents(vae.encode(x), sample_mode="argmax")`` as the
+    img2img pipelines use it.  conv_in reads the image with VaeImageProcessor.preprocess fused (lb_image_conv_in);
+    4 down blocks x 2 resnets; 3 Downsample2D(padding=0) as a patch matrix (lb_im2col_s2_pad01) and one GEMM each; the
+    decoder's mid block (resnet, single-head attention, resnet); GroupNorm + SiLU and conv_out.  quant_conv (1x1, 8 -> 8)
+    and scaling_factor are folded into conv_out's first four output rows in fp32, so the last conv is one N = 8 GEMM
+    producing the scaled mean.  ``dtype``: fp16 or bf16 storage, fp32 accumulation.  One graph-replayed program per
+    image size; ``state_dict``: the diffusers names with ``encoder.`` stripped, plus ``quant_conv.*``."""
+
+    def __init__(self, state_dict, channels, scaling_factor, device, groups=32, dtype=torch.float16,
+                 layers_per_block=2):
+        if dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError(f"VAE encoder dtype must be torch.float16 or torch.bfloat16 (got {dtype})")
+        self.device = torch.device(device)
+        self.dev_index = self.device.index or 0
+        self.channels = tuple(channels)
+        self.scaling_factor = float(scaling_factor)
+        self.groups, self.dtype, self.layers_per_block = groups, dtype, layers_per_block
+        self._plans = {}
+        self.nonfinite = torch.zeros(1, dtype=torch.int32, device=self.device)
+        sd, dev = state_dict, self.device
+
+        def g(n):
+            return sd[n].detach().to(device=dev, dtype=dtype).contiguous()
+
+        def gf(n):
+            return sd[n].detach().to(device=dev, dtype=torch.float32)
+
+        W = self.w = {}
+        W["conv_in.w"] = g("conv_in.weight").permute(2, 3, 1, 0).contiguous()       # [ky][kx][Cin][Cout]
+        W["conv_in.b"] = g("conv_in.bias")
+        for r in [k[: -len(".norm1.weight")] for k in sd if k.endswith(".norm1.weight")]:
+            pack_resnet(W, r, sd, g)
+        for i in range(len(self.channels) - 1):
+            nm = f"down_blocks.{i}.downsamplers.0.conv"
+            W[nm + ".w"], W[nm + ".b"] = pack3(g(nm + ".weight")), g(nm + ".bias")
+        pack_vae_attention(W, "mid_block.attentions.0", sd, g, gf, dtype)
+        W["norm_out.g"], W["norm_out.b"] = g("conv_norm_out.weight"), g("conv_norm_out.bias")
+        # scaling_factor * (quant_conv(conv_out(x)))[:4]: the mean half of the moments, folded in fp32
+        wo, bo = gf("conv_out.weight"), gf("conv_out.bias")                         # [8, C, 3, 3], [8]
+        q = gf("quant_conv.weight").reshape(wo.shape[0], wo.shape[0])[:4]
+        qb = gf("quant_conv.bias")[:4]
+        wm = (self.scaling_factor * (q @ wo.reshape(wo.shape[0], -1))).reshape(4, *wo.shape[1:])
+        bm = self.scaling_factor * (q @ bo + qb)
+        W["conv_out.w8"], W["conv_out.b8"] = pack_conv_out8(wm.permute(0, 2, 3, 1).to(dtype), bm.to(dtype))
+
+    def plan(self, h, w):
+        if (h, w) not in self._plans:
+            self._plans[(h, w)] = _VAEEncoderLowering(self, h, w)
+        return self._plans[(h, w)]
+
+    @torch.no_grad()
+    def encode(self, image_u8):
+        """uint8 [H, W, 3] image on the device (H, W multiples of 8) -> [1, 4, H/8, W/8] scaled posterior mean in
+        the encoder's storage type (a view of the plan's output buffer: the next encode of this size overwrites it)."""
+        assert image_u8.is_cuda and image_u8.dtype == torch.uint8 and image_u8.dim() == 3, \
+            "VAE encode: one uint8 HxWxC CUDA image"
+        H, W_, _ = image_u8.shape
+        if H % 8 or W_ % 8:
+            raise ValueError(f"VAE encode: the image sides must be multiples of 8 (got {W_}x{H})")
+        pl = self.plan(H // 8, W_ // 8)
+        pl.img.copy_(image_u8)
+        pl.prog.run()
+        return pl.x0
+
+    def check_finite(self, x0):
+        """Raise when ``x0`` holds non-finite values: the count comes from lb_add_noise_rows' device counter (no rows
+        written), read once per encode."""
+        from . import ops
+        self.nonfinite.zero_()
+        ops.add_noise_rows(x0, torch.empty(x0.shape, dtype=torch.float16, device=x0.device),
+                           torch.empty((0, 2), dtype=torch.float16, device=x0.device), _cabi.ADD_NOISE_SIGMA,
+                           nonfinite=self.nonfinite)
+        n = int(self.nonfinite.item())
+        if n:
+            if self.dtype == torch.float16:
+                raise _cabi.LB200Error(
+                    f"VAE encode produced {n} non-finite latents: these VAE weights overflow fp16 (the stock SDXL VAE "
+                    "does; its config sets force_upcast); encode in bf16 instead (DiffusersHolder.set_vae_dtype(\"bf16\"), "
+                    "chosen automatically when the VAE config sets force_upcast) or use the fp16-safe SDXL VAE weights "
+                    "(madebyollin/sdxl-vae-fp16-fix)")
+            raise _cabi.LB200Error(f"VAE encode produced {n} non-finite latents in bf16: the VAE weights are not finite")
+
+
+class _VAEEncoderLowering:
+    def __init__(self, enc: VAEEncoderB200, h, w):
+        Wt, dev, groups = enc.w, enc.device, enc.groups
+        act = dict(dtype=enc.dtype, device=dev)
+        ch = list(enc.channels)                       # e.g. [128, 256, 512, 512]
+        B = 1
+        H, W_ = 8 * h, 8 * w
+        P = self.prog = Program(enc.dev_index)
+        self.img = torch.zeros(H, W_, 3, dtype=torch.uint8, device=dev)
+        self.ws = torch.zeros(max(1 << 16, _cabi.load().lb_groupnorm_workspace_bytes(ctx(enc.dev_index), B, H * W_,
+                                                                                      groups)),
+                              dtype=torch.uint8, device=dev)
+        sc = Scratch(enc.dtype, dev)
+
+        def resnet(rname, x, cin, cout, hh, ww, out):
+            lower_resnet(P, Wt, rname, x, cin, cout, B, hh, ww, out, groups, 1e-6, self.ws, sc)
+
+        hh, ww, cin = H, W_, ch[0]
+        x = torch.empty(hh * ww, cin, **act)
+        P.image_conv_in(self.img.view(H * W_, 3), B, H, W_, Wt["conv_in.w"], Wt["conv_in.b"], cin, x)
+        for i, cout in enumerate(ch):
+            for j in range(enc.layers_per_block):
+                out = torch.empty(hh * ww, cout, **act)
+                resnet(f"down_blocks.{i}.resnets.{j}", x, cin, cout, hh, ww, out)
+                x, cin = out, cout
+            nm = f"down_blocks.{i}.downsamplers.0.conv"
+            if (nm + ".w") in Wt:
+                ho, wo = (hh - 2) // 2 + 1, (ww - 2) // 2 + 1
+                cols = sc("im2col", ho * wo, 9 * cout)        # the largest level's patch matrix, reused by the next
+                P.im2col_s2_pad01(x, B, hh, ww, cout, cols)
+                nx = torch.empty(ho * wo, cout, **act)
+                P.gemm(cols, Wt[nm + ".w"], cout, 1, 1, ho * wo, nx, bias=Wt[nm + ".b"])
+                x, hh, ww = nx, ho, wo
+        assert (hh, ww) == (h, w), f"VAE encoder: {H}x{W_} does not reduce to {h}x{w}"
+        C0, S = cin, h * w
+        x2 = torch.empty(S, C0, **act)
+        resnet("mid_block.resnets.0", x, C0, C0, h, w, x2)
+        x3 = torch.empty(S, C0, **act)
+        lower_vae_attention(P, Wt, x2, S, C0, groups, self.ws, sc, x3)
+        x4 = torch.empty(S, C0, **act)
+        resnet("mid_block.resnets.1", x3, C0, C0, h, w, x4)
+        no = sc("n1", S, C0)
+        P.groupnorm(x4, B, S, C0, groups, Wt["norm_out.g"], Wt["norm_out.b"], 1e-6, 1, no, self.ws)
+        self.x0 = torch.empty(1, 4, h, w, **act)
+        lower_conv_out(P, Wt, no, B, h, w, C0, 4, self.x0, sc)
         P.finalize()
