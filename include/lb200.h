@@ -320,6 +320,26 @@ int lb_im2col_s2_pad01(lb_ctx* ctx, const void* x, int64_t ld, int B, int H, int
 int lb_add_noise_rows(lb_ctx* ctx, const void* x0, const void* noise, const void* coeffs_dev, int form, int64_t n,
                       int rows, void* out, int* nonfinite_count_dev, void* stream, int dtype);
 
+/* ---- SDXL T2I-Adapter (diffusers 0.25 T2IAdapter "full_adapter_xl", StableDiffusionXLAdapterPipeline) -----------
+ * lb_add_rows_bcast: dst[b*rows + r, c] = h(dst[b*rows + r, c] + src[r, c]) for b < B, r < rows, c < C (fp16, fp32
+ *   add, h = one fp16 rounding: torch's fp16 ``+=``).  The adapter's per-image state, shared by every batch row (the
+ *   CFG halves, every lockstep job), added in place to a UNet skip or the mid-block output.  dst and src are row-major
+ *   with row strides ld_dst / ld_src (multiples of 8, >= C); C a multiple of 8; bases 16-byte aligned.
+ * lb_pixel_unshuffle_u8: F.pixel_unshuffle(image, r) of a uint8 image [H, W, Cimg] (contiguous, 8-byte aligned base)
+ *   fused with the adapter input's scaling: out [(H/r)*(W/r), r*r*Cimg] fp16 (contiguous), element (i*r + j)*Cimg + c
+ *   of output pixel (y, x) = fp16(float(img[y*r + i, x*r + j, c]) / 255).  The columns are in (i, j, c) order, a
+ *   permutation of torch's (c, i, j): the consumer's weights are permuted to match.  H, W multiples of r; r*Cimg a
+ *   multiple of 8.
+ * lb_avgpool2_ceil: AvgPool2d(2, stride 2, ceil_mode=True) of an NHWC fp16 map [H*W, C] (row stride ld) into
+ *   [ceil(H/2)*ceil(W/2), C] (row stride ldo): the fp32 sum of the window's in-bounds pixels in row-major order
+ *   divided by their count, one fp16 rounding (torch's avg_pool2d).  C and the strides multiples of 8.
+ */
+int lb_add_rows_bcast(lb_ctx* ctx, void* dst, int64_t ld_dst, const void* src, int64_t ld_src, int B, int64_t rows,
+                      int C, void* stream);
+int lb_pixel_unshuffle_u8(lb_ctx* ctx, const void* img_u8, int H, int W, int Cimg, int r, void* out, void* stream);
+int lb_avgpool2_ceil(lb_ctx* ctx, const void* x, int64_t ld, int H, int W, int C, void* out, int64_t ldo,
+                     void* stream);
+
 /* ---- VAE decoder helpers (SURVEY section 8f next #1; latent2image, diffusers_holder.py:114-143) ----
  * lb_latent_prep: post_quant_conv(latents / scaling_factor) as a per-pixel CxC fp32 matrix (scale folded in).
  * lb_softmax_rows: row softmax of an fp16 matrix (the VAE mid-block single-head attention, head dim 512,
@@ -388,13 +408,17 @@ int lb_frames_lerp_u8(lb_ctx* ctx, const void* frames_u8, int64_t n, const int* 
  * w, bias, Cout, out, ld_out, stride, in_u8 and act as lb_cond_conv's ``silu``.
  * LB_OP_IMAGE_CONV_IN (lb_image_conv_in) uses the ``conv`` member's x, ld_x, B, Cin, H, W, w, bias, Cout, out and
  * ld_out, with lb_op.dtype; LB_OP_IM2COL_S2_PAD01 (lb_im2col_s2_pad01) uses ``resample`` like LB_OP_IM2COL_S2.
+ * LB_OP_ADD_ROWS_BCAST (lb_add_rows_bcast) uses ``aux``: out = dst, ld_out = ld_dst, x = src, ld_x = ld_src, B,
+ * n = rows, C.  LB_OP_PIXEL_UNSHUFFLE_U8 (lb_pixel_unshuffle_u8) uses ``patch``: x = image, H, W, C = Cimg, k = r, out.
+ * LB_OP_AVGPOOL2_CEIL (lb_avgpool2_ceil) uses ``patch`` like LB_OP_MAXPOOL3S2: x, ld_x, H, W, C, out, ld_out.
  */
 enum {
     LB_OP_GEMM = 1, LB_OP_ATTENTION = 2, LB_OP_GROUPNORM = 3, LB_OP_LAYERNORM = 4, LB_OP_EMBED_INPUTS = 5,
     LB_OP_LINEAR_SMALL = 6, LB_OP_CONV_IN = 7, LB_OP_UPSAMPLE_NEAREST = 9, LB_OP_IM2COL_S2 = 10,
     LB_OP_LATENT_PREP = 11, LB_OP_SOFTMAX_ROWS = 12, LB_OP_POSTPROCESS_U8 = 13,
     LB_OP_LPIPS_IM2COL_U8 = 14, LB_OP_IM2COL = 15, LB_OP_MAXPOOL3S2 = 16, LB_OP_NHWC_TO_NCHW = 17,
-    LB_OP_CONV_IN_ADD = 19, LB_OP_COND_CONV = 20, LB_OP_IMAGE_CONV_IN = 21, LB_OP_IM2COL_S2_PAD01 = 22
+    LB_OP_CONV_IN_ADD = 19, LB_OP_COND_CONV = 20, LB_OP_IMAGE_CONV_IN = 21, LB_OP_IM2COL_S2_PAD01 = 22,
+    LB_OP_ADD_ROWS_BCAST = 23, LB_OP_PIXEL_UNSHUFFLE_U8 = 24, LB_OP_AVGPOOL2_CEIL = 25
 };
 typedef struct lb_op {
     int32_t kind;

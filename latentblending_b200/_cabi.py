@@ -105,6 +105,7 @@ OP_GEMM, OP_ATTENTION, OP_GROUPNORM, OP_LAYERNORM, OP_EMBED_INPUTS, OP_LINEAR_SM
 (OP_UPSAMPLE_NEAREST, OP_IM2COL_S2, OP_LATENT_PREP, OP_SOFTMAX_ROWS, OP_POSTPROCESS_U8, OP_LPIPS_IM2COL_U8, OP_IM2COL,
  OP_MAXPOOL3S2, OP_NHWC_TO_NCHW) = 9, 10, 11, 12, 13, 14, 15, 16, 17
 OP_CONV_IN_ADD, OP_COND_CONV, OP_IMAGE_CONV_IN, OP_IM2COL_S2_PAD01 = 19, 20, 21, 22
+OP_ADD_ROWS_BCAST, OP_PIXEL_UNSHUFFLE_U8, OP_AVGPOOL2_CEIL = 23, 24, 25
 ADD_NOISE_SIGMA, ADD_NOISE_ALPHA_SIGMA = 0, 1   # lb_add_noise_rows' form: x0 + b*noise, a*x0 + b*noise
 CONV_IN_PLAIN, CONV_IN_TINY_VAE = 0, 1     # lb_conv_in's act
 
@@ -159,6 +160,9 @@ SIGNATURES = {
     "lb_im2col_s2_pad01": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "lb_add_noise_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p,
                                   c_void_p, c_int]),
+    "lb_add_rows_bcast": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int, c_int64, c_int, c_void_p]),
+    "lb_pixel_unshuffle_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "lb_avgpool2_ceil": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
     "lb_upsample_nearest": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
                                     c_int, c_void_p, c_int]),
     "lb_im2col_s2": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

@@ -173,6 +173,15 @@ class BlendingEngine():
         ``control_guidance_start`` and ``control_guidance_end``.  Raises ValueError for a pipe without a ControlNet."""
         self.dh.set_control_image(image, conditioning_scale, guidance_start, guidance_end)
 
+    def set_adapter_image(self, image, conditioning_scale=1.0, conditioning_factor=1.0):
+        """Hold the transition's structure with the pipe's SDXL T2I-Adapter: ``image`` (a PIL image, or an HxWx3 /
+        HxW uint8 array: a depth, canny, sketch, lineart or pose map) conditions every branch of the tree; ``None``
+        switches it off.  The arguments follow StableDiffusionXLAdapterPipeline's ``adapter_conditioning_scale`` and
+        ``adapter_conditioning_factor`` (the leading fraction of the steps that get the features).  The features are
+        computed once per image and size, not per step.  Raises ValueError for a pipe without an adapter and for an
+        output size whose sides are not multiples of 16."""
+        self.dh.set_adapter_image(image, conditioning_scale, conditioning_factor)
+
     def set_prompt1(self, prompt: str):
         prompt = prompt.replace("_", " ")
         self.prompt1 = prompt

@@ -3,6 +3,7 @@
 //       (time_embedding, add_embedding, all resnet time_emb_proj in one batched launch)
 //   K2  conv_in  (4 -> C0, 3x3, NCHW latent in, NHWC out)
 //       nearest upsample (2x, or 2x cropped by one row / column), stride-2 im2col (the two Downsample2D convs then run as plain GEMMs)
+//       the T2I-Adapter's pixel unshuffle and ceil-mode 2x2 average pool, and its in-place state add
 // Replace pieces of pipe.unet(...) (call site latentblending/diffusers_holder.py:336-344;
 // diffusers 0.25.0 embeddings.py / resnet.py / unet_2d_condition.py).
 #include "common.cuh"
@@ -259,6 +260,96 @@ im2col_s2_kernel(const __half* __restrict__ x, long long ld, int B, int H, int W
     }
 }
 
+// ---- T2I-Adapter pieces -------------------------------------------------------------------------------------------
+// add_rows_bcast: dst[b*rows + r, :C] += src[r, :C] for every batch row b: the adapter's per-image state added in
+// place to a skip (or the mid output) of every CFG half / lockstep job.  fp32 add, one rounding: torch's fp16 ``+=``.
+__global__ void __launch_bounds__(kThreads)
+add_rows_bcast_kernel(__half* __restrict__ dst, long long ld_dst, const __half* __restrict__ src, long long ld_src,
+                      int B, long long rows, int C) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int vecs = C >> 3;
+    const long long total = (long long)B * rows * vecs;
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
+        const int v = (int)(i % vecs);
+        const long long row = i / vecs, r = row % rows;
+        uint4* d = reinterpret_cast<uint4*>(dst + row * ld_dst + v * 8);
+        uint4 a = *d;
+        const uint4 s = *reinterpret_cast<const uint4*>(src + r * ld_src + v * 8);
+        __half2* ah = reinterpret_cast<__half2*>(&a);
+        const __half2* sh = reinterpret_cast<const __half2*>(&s);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 x = __half22float2(ah[j]), y = __half22float2(sh[j]);
+            ah[j] = __floats2half2_rn(x.x + y.x, x.y + y.y);
+        }
+        *d = a;
+    }
+}
+
+// pixel_unshuffle_u8: uint8 image [H, W, Cimg] -> fp16 [(H/r)*(W/r), r*r*Cimg], fp16(float(u) / 255), columns in
+// (i, j, c) order (i, j the offset inside the r x r block).  Row i of a block is r*Cimg consecutive image bytes, so
+// each thread converts 8 consecutive bytes into one 16-byte store.  F.pixel_unshuffle's (c, i, j) order is the
+// caller's weight permutation.
+__global__ void __launch_bounds__(kThreads)
+pixel_unshuffle_u8_kernel(const uint8_t* __restrict__ img, int H, int W, int Cimg, int r, __half* __restrict__ out) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int Wo = W / r, seg = r * Cimg, K = seg * r, vecs = K >> 3;
+    const long long total = (long long)(H / r) * Wo * vecs;
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
+        const int v = (int)(i % vecs);
+        const long long opix = i / vecs;
+        const int xo = (int)(opix % Wo), yo = (int)(opix / Wo);
+        const int col = v * 8, bi = col / seg, off = col % seg;
+        const uint2 raw = *reinterpret_cast<const uint2*>(img + ((long long)(yo * r + bi) * W + (long long)xo * r) * Cimg + off);
+        const uint8_t* b = reinterpret_cast<const uint8_t*>(&raw);
+        uint4 o;
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn((float)b[2 * j] / 255.0f, (float)b[2 * j + 1] / 255.0f);
+        *reinterpret_cast<uint4*>(out + opix * K + col) = o;
+    }
+}
+
+// avgpool2_ceil: NHWC AvgPool2d(2, stride 2, ceil_mode=True, padding 0): Ho = ceil(H/2); a window hanging over the
+// bottom / right edge is clipped and divided by its in-bounds count.  fp32 sum in row-major window order, then the
+// division, one rounding: torch's avg_pool2d on fp16.
+__global__ void __launch_bounds__(kThreads)
+avgpool2_ceil_kernel(const __half* __restrict__ x, long long ld, int H, int W, int C, __half* __restrict__ out,
+                     long long ldo) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2, vecs = C >> 3;
+    const long long total = (long long)Ho * Wo * vecs;
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
+        const int v = (int)(i % vecs);
+        const long long opix = i / vecs;
+        const int xo = (int)(opix % Wo), yo = (int)(opix / Wo);
+        const int y1 = min(2 * yo + 2, H), x1 = min(2 * xo + 2, W);
+        float acc[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+        for (int y = 2 * yo; y < y1; ++y)
+            for (int xx = 2 * xo; xx < x1; ++xx) {
+                const uint4 q = *reinterpret_cast<const uint4*>(x + ((long long)y * W + xx) * ld + v * 8);
+                const __half2* qh = reinterpret_cast<const __half2*>(&q);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 f = __half22float2(qh[j]);
+                    acc[2 * j] += f.x;
+                    acc[2 * j + 1] += f.y;
+                }
+            }
+        const float cnt = (float)((y1 - 2 * yo) * (x1 - 2 * xo));
+        uint4 o;
+        __half2* oh = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(acc[2 * j] / cnt, acc[2 * j + 1] / cnt);
+        *reinterpret_cast<uint4*>(out + opix * ldo + v * 8) = o;
+    }
+}
+
 unsigned grid_for(long long work_items, int sm) {
     long long g = lb_ceil_div(work_items, kThreads);
     const long long cap = (long long)sm * 8;
@@ -402,6 +493,50 @@ extern "C" int lb_im2col_s2_pad01(lb_ctx* ctx, const void* x, int64_t ld, int B,
     const long long total = (long long)B * ((H - 2) / 2 + 1) * ((W - 2) / 2 + 1) * 9 * (C / 8);
     lb_launch_pdl(im2col_s2_kernel<0>, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream),
                   (const __half*)x, ld, B, H, W, C, (__half*)out);
+    LB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int lb_add_rows_bcast(lb_ctx* ctx, void* dst, int64_t ld_dst, const void* src, int64_t ld_src, int B,
+                                 int64_t rows, int C, void* stream) {
+    LB_REQUIRE(ctx && dst && src, "lb_add_rows_bcast: null argument");
+    LB_REQUIRE(B >= 1 && rows >= 1 && C >= 8 && C % 8 == 0 && ld_dst % 8 == 0 && ld_src % 8 == 0 && ld_dst >= C &&
+               ld_src >= C && lb_aligned16(dst) && lb_aligned16(src),
+               "lb_add_rows_bcast: needs B, rows >= 1, C a multiple of 8, row strides >= C and multiples of 8, bases "
+               "16-byte aligned (got B %d rows %lld C %d ld_dst %lld ld_src %lld)", B, (long long)rows, C,
+               (long long)ld_dst, (long long)ld_src);
+    const long long total = (long long)B * rows * (C / 8);
+    lb_launch_pdl(add_rows_bcast_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream), (__half*)dst,
+                  (long long)ld_dst, (const __half*)src, (long long)ld_src, B, (long long)rows, C);
+    LB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int lb_pixel_unshuffle_u8(lb_ctx* ctx, const void* img_u8, int H, int W, int Cimg, int r, void* out,
+                                     void* stream) {
+    LB_REQUIRE(ctx && img_u8 && out, "lb_pixel_unshuffle_u8: null argument");
+    LB_REQUIRE(Cimg >= 1 && r >= 1 && (r * Cimg) % 8 == 0 && H >= r && W >= r && H % r == 0 && W % r == 0,
+               "lb_pixel_unshuffle_u8: needs H, W multiples of r and r*Cimg a multiple of 8 (got H %d W %d Cimg %d "
+               "r %d)", H, W, Cimg, r);
+    LB_REQUIRE((reinterpret_cast<uintptr_t>(img_u8) & 7u) == 0 && lb_aligned16(out),
+               "lb_pixel_unshuffle_u8: the image base must be 8-byte and the output base 16-byte aligned");
+    const long long total = (long long)(H / r) * (W / r) * (r * r * Cimg / 8);
+    lb_launch_pdl(pixel_unshuffle_u8_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream),
+                  (const uint8_t*)img_u8, H, W, Cimg, r, (__half*)out);
+    LB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int lb_avgpool2_ceil(lb_ctx* ctx, const void* x, int64_t ld, int H, int W, int C, void* out, int64_t ldo,
+                                void* stream) {
+    LB_REQUIRE(ctx && x && out, "lb_avgpool2_ceil: null argument");
+    LB_REQUIRE(H >= 1 && W >= 1 && C >= 8 && C % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0 && ld >= C && ldo >= C &&
+               lb_aligned16(x) && lb_aligned16(out),
+               "lb_avgpool2_ceil: needs C a multiple of 8, row strides >= C and multiples of 8, bases 16-byte aligned "
+               "(got H %d W %d C %d ld %lld ldo %lld)", H, W, C, (long long)ld, (long long)ldo);
+    const long long total = (long long)((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
+    lb_launch_pdl(avgpool2_ceil_kernel, grid_for(total, ctx->sm_count), kThreads, 0, lb_stream(stream),
+                  (const __half*)x, (long long)ld, H, W, C, (__half*)out, (long long)ldo);
     LB_LAUNCH_CHECK();
     return 0;
 }

@@ -97,6 +97,7 @@ extern "C" int lb_program_create(lb_ctx* ctx, const lb_op* ops, int64_t n_ops, l
             case LB_OP_LATENT_PREP: case LB_OP_SOFTMAX_ROWS: case LB_OP_POSTPROCESS_U8:
             case LB_OP_LPIPS_IM2COL_U8: case LB_OP_IM2COL: case LB_OP_MAXPOOL3S2: case LB_OP_NHWC_TO_NCHW:
             case LB_OP_IMAGE_CONV_IN: case LB_OP_IM2COL_S2_PAD01:
+            case LB_OP_ADD_ROWS_BCAST: case LB_OP_PIXEL_UNSHUFFLE_U8: case LB_OP_AVGPOOL2_CEIL:
                 break;
             case LB_OP_CONV_IN_ADD: case LB_OP_COND_CONV:
                 if (ops[i].kind == LB_OP_CONV_IN_ADD && ops[i].u.conv.act != 0) {
@@ -310,6 +311,21 @@ static int program_launch_all(lb_program* prog, float t, const float* t_dev, uin
             case LB_OP_MAXPOOL3S2: {
                 const auto& a = o.u.patch;
                 e = lb_maxpool3s2(ctx, a.x, a.ld_x, a.H, a.W, a.C, a.out, a.ld_out, stream);
+                break;
+            }
+            case LB_OP_ADD_ROWS_BCAST: {
+                const auto& a = o.u.aux;
+                e = lb_add_rows_bcast(ctx, a.out, a.ld_out, a.x, a.ld_x, a.B, a.n, a.C, stream);
+                break;
+            }
+            case LB_OP_PIXEL_UNSHUFFLE_U8: {
+                const auto& a = o.u.patch;
+                e = lb_pixel_unshuffle_u8(ctx, a.x, a.H, a.W, a.C, a.k, a.out, stream);
+                break;
+            }
+            case LB_OP_AVGPOOL2_CEIL: {
+                const auto& a = o.u.patch;
+                e = lb_avgpool2_ceil(ctx, a.x, a.ld_x, a.H, a.W, a.C, a.out, a.ld_out, stream);
                 break;
             }
         }

@@ -54,7 +54,14 @@ class DiffusersHolder:
             from .controlnet import COND_CHANNELS, ControlNetB200
             self.controlnet = ControlNetB200(pipe.controlnet_cfg, pipe.controlnet_state_dict, self.device,
                                              getattr(pipe, "controlnet_cond_channels", None) or COND_CHANNELS)
-        self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device, controlnet=self.controlnet)
+        # an SDXL T2I-Adapter (pipe.adapter of a StableDiffusionXLAdapterPipeline): its features are computed once per
+        # image and size, and every UNet plan records a step program that adds them, run while an adapter image is set
+        self.adapter, self.adapter_cond = None, None
+        if getattr(pipe, "adapter_state_dict", None) is not None:
+            from .t2i_adapter import AdapterB200
+            self.adapter = AdapterB200(pipe.adapter_cfg, pipe.adapter_state_dict, self.device, pipe.vae_scale_factor)
+        self.unet = UNetB200(pipe.unet_cfg, pipe.unet_state_dict, self.device, controlnet=self.controlnet,
+                             adapter=self.adapter)
         self.vae = None
         self.vae_encoder = None       # built on the first image2latent, in the decoder's storage type
         self.set_vae_dtype(getattr(pipe, "vae_dtype", "fp16"))
@@ -158,6 +165,63 @@ class DiffusersHolder:
             return False
         from .controlnet import keep_scale
         return keep_scale(i, num_steps, c["start"], c["end"]) * c["scale"] > 0
+
+    def set_adapter_image(self, image, conditioning_scale=1.0, conditioning_factor=1.0):
+        """Condition every following denoise on ``image`` (a PIL image, or an HxWx3 / HxW uint8 array) through the
+        pipe's T2I-Adapter; ``None`` switches the adapter off.  The arguments are StableDiffusionXLAdapterPipeline's
+        ``adapter_conditioning_scale`` and ``adapter_conditioning_factor``: the adapter's features, times
+        ``conditioning_scale``, are added at the steps i < int(N * conditioning_factor) of N.  The image is converted to
+        the adapter's mode ("RGB" or "L") and resized with LANCZOS to the output size, whose sides must be multiples of
+        16; the features are computed once per image, scale and size."""
+        if self.adapter is None:
+            raise ValueError("set_adapter_image needs a pipe with a T2I-Adapter (StableDiffusionXLAdapterPipeline, or "
+                             "SyntheticSDXLPipe(adapter=...))")
+        if image is None:
+            self.adapter_cond = None
+            return
+        if not 0.0 <= conditioning_factor <= 1.0:
+            raise ValueError(f"conditioning_factor must be in [0, 1] (got {conditioning_factor})")
+        from PIL import Image
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.uint8 or not (image.ndim == 2 or (image.ndim == 3 and image.shape[2] == 3)):
+                raise ValueError(f"an adapter image array must be HxWx3 or HxW uint8 (got {image.dtype} {image.shape})")
+            image = Image.fromarray(image)
+        elif not isinstance(image, Image.Image):
+            raise TypeError(f"the adapter image must be a PIL image or a uint8 array (got {type(image)})")
+        mode = "RGB" if self.adapter.in_channels == 3 else "L"
+        self.adapter_cond = dict(image=image.convert(mode), scale=float(conditioning_scale),
+                                 factor=float(conditioning_factor), computed=set())
+        self._refresh_adapter(self.height_latent, self.width_latent)
+
+    def _refresh_adapter(self, h, w):
+        """Compute the adapter's scaled states for latent size (h, w) unless the current image already has them."""
+        a = self.adapter_cond
+        if (h, w) in a["computed"]:
+            return
+        from PIL import Image
+        from .t2i_adapter import check_image_size
+        s = self.pipe.vae_scale_factor
+        check_image_size(h * s, w * s)
+        arr = np.array(a["image"].resize((w * s, h * s), resample=Image.LANCZOS))
+        self.adapter.compute(torch.from_numpy(np.ascontiguousarray(arr)).to(self.device), h, w, a["scale"])
+        a["computed"].add((h, w))
+
+    def adapter_active(self, i, num_steps):
+        """Whether step ``i`` of ``num_steps`` runs the UNet step program with the adapter's states added."""
+        a = self.adapter_cond
+        if a is None or a["scale"] == 0:
+            return False
+        from .t2i_adapter import adapter_steps
+        return i < adapter_steps(num_steps, a["factor"])
+
+    def step_program(self, plan, i, num_steps):
+        """The step program of ``plan`` that step ``i`` of ``num_steps`` runs: with the ControlNet, with the adapter,
+        or plain."""
+        if self.control_active(i, num_steps):
+            return plan.prog_step_cn
+        if self.adapter_active(i, num_steps):
+            return plan.prog_step_ad
+        return plan.prog_step
 
     def set_negative_prompt(self, negative_prompt):
         self.negative_prompt = [negative_prompt] if isinstance(negative_prompt, str) else negative_prompt
@@ -370,6 +434,8 @@ class DiffusersHolder:
             plan.prog_ctx.run()                                # cross-attention K/V: once per conditioning
         if self.control is not None:
             self._embed_control(h, w)
+        if self.adapter_cond is not None:
+            self._refresh_adapter(h, w)
         n = C * h * w
         outs = [[None] * N for _ in jobs]
         trajs = [torch.empty((N, C, h, w), dtype=torch.float16, device=self.device) for _ in jobs]
@@ -418,16 +484,15 @@ class DiffusersHolder:
                     scaled[j] = False
                 if not scaled[j]:
                     ops.scale_model_input(latents[j], Bj, sc["divisor"], out=x_in[j * Bj:(j + 1) * Bj])
-            control = self.control_active(i, N)
             if dual is None:
-                (plan.prog_step_cn if control else plan.prog_step).run(sc["t"])
+                self.step_program(plan, i, N).run(sc["t"])
             else:
                 main = torch.cuda.current_stream()
                 dual["fork"].record(main)
                 for pl, st, ev in zip(dual["plans"], dual["streams"], dual["done"]):
                     st.wait_event(dual["fork"])
                     with torch.cuda.stream(st):
-                        (pl.prog_step_cn if control else pl.prog_step).run(sc["t"])
+                        self.step_program(pl, i, N).run(sc["t"])
                         ev.record(st)
                 for ev in dual["done"]:
                     main.wait_event(ev)

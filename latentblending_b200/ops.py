@@ -344,6 +344,30 @@ def image_conv_in(img_u8, w_packed, bias, Cout, out=None):
     return out
 
 
+def add_rows_bcast(dst, src, B):
+    """fp16 ``dst[b*rows + r] += src[r]`` in place for every batch row b (lb_add_rows_bcast); returns ``dst``."""
+    _run1(_dev(dst), lambda P: P.add_rows_bcast(dst, src, B))
+    return dst
+
+
+def pixel_unshuffle_u8(img_u8, r, out=None):
+    """uint8 [H, W, Cimg] -> fp16 [(H/r)*(W/r), r*r*Cimg] = u / 255, columns in (i, j, c) order
+    (lb_pixel_unshuffle_u8)."""
+    H, W, C = img_u8.shape
+    if out is None:
+        out = torch.empty(((H // r) * (W // r), r * r * C), dtype=torch.float16, device=img_u8.device)
+    _run1(_dev(img_u8), lambda P: P.pixel_unshuffle_u8(img_u8, r, out))
+    return out
+
+
+def avgpool2_ceil(x, H, W, C, out=None):
+    """AvgPool2d(2, 2, ceil_mode=True) of NHWC fp16 rows [H*W, >=C] -> [ceil(H/2)*ceil(W/2), C] (lb_avgpool2_ceil)."""
+    if out is None:
+        out = torch.empty((((H + 1) // 2) * ((W + 1) // 2), C), dtype=torch.float16, device=x.device)
+    _run1(_dev(x), lambda P: P.avgpool2_ceil(x, H, W, C, out))
+    return out
+
+
 def add_noise_rows(x0, noise, coeffs, form, out=None, nonfinite=None):
     """out[r] = add_noise(x0, noise, coeffs[r]) (lb_add_noise_rows): ``x0`` fp16 / bf16 and ``noise`` fp16 with n
     elements each, ``coeffs`` a device fp16 [rows, 2] of (a, b), ``form`` _cabi.ADD_NOISE_SIGMA (x0 + b*noise) or

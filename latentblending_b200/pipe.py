@@ -167,6 +167,46 @@ def random_controlnet_state_dict(cfg: UNetConfig, seed, device, damp=0.1):
     return sd
 
 
+def adapter_param_shapes(in_channels=3, channels=(320, 640, 1280, 1280), num_res_blocks=2, downscale_factor=16):
+    """diffusers state_dict names -> shapes of an SDXL T2IAdapter (``adapter_type="full_adapter_xl"``): conv_in on
+    the pixel-unshuffled image, then four AdapterBlocks (t2i_adapter.body_layout), a 1x1 in_conv where the channel
+    count changes and ``num_res_blocks`` resnets of a 3x3 block1 and a 1x1 block2 each."""
+    from .t2i_adapter import body_layout
+    P = OrderedDict()
+    P["adapter.conv_in.weight"] = (channels[0], in_channels * downscale_factor ** 2, 3, 3)
+    P["adapter.conv_in.bias"] = (channels[0],)
+    for i, (ci, co, _) in enumerate(body_layout(channels)):
+        if ci != co:
+            P[f"adapter.body.{i}.in_conv.weight"], P[f"adapter.body.{i}.in_conv.bias"] = (co, ci, 1, 1), (co,)
+        for j in range(num_res_blocks):
+            q = f"adapter.body.{i}.resnets.{j}"
+            P[q + ".block1.weight"], P[q + ".block1.bias"] = (co, co, 3, 3), (co,)
+            P[q + ".block2.weight"], P[q + ".block2.bias"] = (co, co, 1, 1), (co,)
+    return P
+
+
+def random_adapter_state_dict(cfg, seed, device, damp=0.1):
+    """Seeded T2I-Adapter weights (``cfg``: the T2IAdapter config keys) with ``random_state_dict``'s recipe.  Every
+    block2 is damped like the other residual branches, but not zeroed, so the features change the UNet's output."""
+    shapes = adapter_param_shapes(cfg["in_channels"], cfg["channels"], cfg["num_res_blocks"], cfg["downscale_factor"])
+    sd = random_state_dict(shapes, seed, device, damp=damp)
+    for k in sd:
+        if ".block2." in k:
+            sd[k] = (sd[k].float() * damp).to(sd[k].dtype)
+    return sd
+
+
+# SyntheticSDXLPipe seeds its T2I-Adapter weights with seed + this offset: no other synthetic state dict uses it
+ADAPTER_SEED_OFFSET = 5003
+
+
+def adapter_config(unet_cfg: UNetConfig, in_channels):
+    """The T2IAdapter config of an SDXL adapter for ``unet_cfg``: channels = block_out_channels + the last again."""
+    ch = tuple(unet_cfg.block_out_channels)
+    return dict(in_channels=in_channels, channels=ch + ch[-1:], num_res_blocks=2, downscale_factor=16,
+                adapter_type="full_adapter_xl")
+
+
 def vae_param_shapes(channels=VAE_CHANNELS, latent=4):
     P = OrderedDict()
     ch = list(reversed(channels))
@@ -351,7 +391,7 @@ class SyntheticSDXLPipe:
     def __init__(self, name="stabilityai/stable-diffusion-xl-base-1.0", device="cuda:0", unet_cfg: UNetConfig = None,
                  seed=0, unet_state_dict=None, vae_state_dict=None, vae_channels=VAE_CHANNELS,
                  lpips_state_dict=None, vae_dtype="fp16", vae="kl", scheduler=None, controlnet=None,
-                 controlnet_state_dict=None, vae_encoder_state_dict=None):
+                 controlnet_state_dict=None, vae_encoder_state_dict=None, adapter=None, adapter_state_dict=None):
         """``scheduler``: None (Euler for SDXL base, Euler-ancestral for a name with "turbo"), "euler",
         "euler_ancestral", "lcm" (LCMScheduler tables: LCM-LoRA-style with the base UNet, LCM-SDXL-style with
         ``unet_cfg.time_cond_proj_dim`` set) or one of DPM_SCHEDULERS (DPMSolverMultistepScheduler tables for the SDXL
@@ -363,13 +403,20 @@ class SyntheticSDXLPipe:
         ``controlnet``: None, "full" or "small" (``controlnet_config``): an SDXL ControlNet with seeded weights
         (``random_controlnet_state_dict``) unless ``controlnet_state_dict`` is given.
         ``vae_encoder_state_dict``: the KL VAE's encoder + quant_conv weights (``vae_encoder_param_shapes``), seeded
-        with ``seed + VAE_ENCODER_SEED_OFFSET`` when omitted; a tiny-VAE pipe has no encoder."""
+        with ``seed + VAE_ENCODER_SEED_OFFSET`` when omitted; a tiny-VAE pipe has no encoder.
+        ``adapter``: None, "rgb" or "gray": an SDXL T2I-Adapter taking 3 or 1 image channels (``adapter_config``) with
+        weights seeded with ``seed + ADAPTER_SEED_OFFSET`` (``random_adapter_state_dict``) unless
+        ``adapter_state_dict`` is given.  Not together with a ControlNet."""
         if vae_dtype not in VAE_DTYPES:
             raise ValueError(f"vae_dtype must be one of {sorted(VAE_DTYPES)} (got {vae_dtype!r})")
         if vae not in ("kl", "tiny"):
             raise ValueError(f"vae must be 'kl' or 'tiny' (got {vae!r})")
         if vae == "tiny" and vae_dtype != "fp16":
             raise ValueError("the tiny VAE decoder runs in fp16 only (vae_dtype='fp16')")
+        if adapter not in (None, "rgb", "gray"):
+            raise ValueError(f"adapter must be None, 'rgb' or 'gray' (got {adapter!r})")
+        if adapter is not None and controlnet is not None:
+            raise ValueError("a ControlNet and a T2I-Adapter together are not supported")
         if scheduler not in (None, "euler", "euler_ancestral", "lcm", *DPM_SCHEDULERS):
             raise ValueError(f"scheduler must be None, 'euler', 'euler_ancestral', 'lcm' or one of "
                              f"{sorted(DPM_SCHEDULERS)} (got {scheduler!r})")
@@ -416,6 +463,11 @@ class SyntheticSDXLPipe:
                 random_controlnet_state_dict(self.controlnet_cfg, seed + 2, self.device)
         self.controlnet_cond_channels = None          # the default, controlnet.COND_CHANNELS
         self.controlnet_bgr = False
+        self.adapter_cfg = self.adapter_state_dict = None
+        if adapter is not None:
+            self.adapter_cfg = adapter_config(self.unet_cfg, 3 if adapter == "rgb" else 1)
+            self.adapter_state_dict = adapter_state_dict if adapter_state_dict is not None else \
+                random_adapter_state_dict(self.adapter_cfg, seed + ADAPTER_SEED_OFFSET, self.device)
 
     def encode_prompt(self, prompt, negative_prompt=None, do_classifier_free_guidance=True, dtype=torch.float16):
         """Synthetic stand-in for StableDiffusionXLPipeline.encode_prompt (diffusers_holder.py:81-95)."""
@@ -507,6 +559,7 @@ class DiffusersSDXLPipe:
             raise ValueError(f"the pipeline's UNet holds unfused LoRA layers ({len(lora)} keys, e.g. {lora[0]!r}): "
                              "fuse them into the weights first with pipe.fuse_lora(); pipe.unload_lora_weights()")
         self._take_controlnet(getattr(pipe, "controlnet", None))
+        self._take_adapter(getattr(pipe, "adapter", None))
         vsd = pipe.vae.state_dict()
         vcfg = pipe.vae.config
         if type(pipe.vae).__name__ == "AutoencoderTiny":
@@ -580,6 +633,46 @@ class DiffusersSDXLPipe:
                              f"{tuple(sd[bad[0]].shape)} vs {want[bad[0]]}")
         self.controlnet_cfg, self.controlnet_state_dict = ccfg, sd
         self.controlnet_cond_channels, self.controlnet_bgr = cond, order == "bgr"
+
+    def _take_adapter(self, ad):
+        """A StableDiffusionXLAdapterPipeline's ``adapter`` (one T2IAdapter of type "full_adapter_xl"): its config and
+        its state dict, every key of which the lowering must represent."""
+        self.adapter_cfg = self.adapter_state_dict = None
+        if ad is None:
+            return
+        if type(ad).__name__ == "MultiAdapter" or isinstance(ad, (list, tuple)):
+            raise ValueError("several T2I-Adapters at once (MultiAdapter) are not supported")
+        if self.controlnet_state_dict is not None:
+            raise ValueError("a pipeline with both a ControlNet and a T2I-Adapter is not supported")
+        c = ad.config
+
+        def get(k, default=None):
+            return c[k] if k in c else getattr(c, k, default)
+        kind = get("adapter_type", "full_adapter")
+        if kind != "full_adapter_xl":
+            raise ValueError(f"only the SDXL T2I-Adapter (adapter_type 'full_adapter_xl') is supported, not {kind!r}")
+        cin = int(get("in_channels", 3))
+        if cin not in (1, 3):
+            raise ValueError(f"the T2I-Adapter takes {cin} image channels; only 1 or 3 are supported")
+        cfg = dict(in_channels=cin, channels=tuple(get("channels")), num_res_blocks=int(get("num_res_blocks", 2)),
+                   downscale_factor=int(get("downscale_factor", 16)), adapter_type=kind)
+        if cfg["downscale_factor"] != 16:
+            raise ValueError(f"the T2I-Adapter's downscale_factor is {cfg['downscale_factor']}; SDXL's is 16")
+        ch = tuple(self.unet_cfg.block_out_channels)
+        if len(ch) != 3 or cfg["channels"] != ch + ch[-1:]:
+            raise ValueError(f"the T2I-Adapter's channels {cfg['channels']} do not match the UNet's "
+                             f"block_out_channels {ch} followed by the last one again")
+        sd = ad.state_dict()
+        want = adapter_param_shapes(cin, cfg["channels"], cfg["num_res_blocks"], cfg["downscale_factor"])
+        extra, missing = sorted(set(sd) - set(want)), sorted(set(want) - set(sd))
+        if extra or missing:
+            raise ValueError(f"the T2I-Adapter's layout is not one this lowering represents: {len(extra)} unexpected "
+                             f"keys (e.g. {extra[:3]}), {len(missing)} missing (e.g. {missing[:3]})")
+        bad = [k for k, shp in want.items() if tuple(sd[k].shape) != shp]
+        if bad:
+            raise ValueError(f"the T2I-Adapter's parameter shapes differ from its config's, e.g. {bad[0]!r}: "
+                             f"{tuple(sd[bad[0]].shape)} vs {want[bad[0]]}")
+        self.adapter_cfg, self.adapter_state_dict = cfg, sd
 
     def encode_prompt(self, prompt, negative_prompt=None, do_classifier_free_guidance=True, dtype=torch.float16):
         """diffusers_holder.py:79-96: the pipeline's own encode_prompt (both CLIP encoders), 4-tuple out."""

@@ -7,11 +7,11 @@ import ctypes
 import torch
 
 from . import _cabi
-from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ATTENTION, OP_COND_CONV, OP_CONV_IN, OP_CONV_IN_ADD,
+from ._cabi import (GEMM_RELU, GEMM_STATIC_W, OP_ADD_ROWS_BCAST, OP_ATTENTION, OP_AVGPOOL2_CEIL, OP_COND_CONV, OP_CONV_IN, OP_CONV_IN_ADD,
                     OP_EMBED_INPUTS, OP_GEMM, OP_IMAGE_CONV_IN, OP_IM2COL_S2_PAD01,
                     OP_GROUPNORM, OP_IM2COL, OP_IM2COL_S2, OP_LATENT_PREP, OP_LAYERNORM, OP_LINEAR_SMALL,
-                    OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_POSTPROCESS_U8, OP_SOFTMAX_ROWS,
-                    OP_UPSAMPLE_NEAREST, Op, check, ctx, stream_ptr)
+                    OP_LPIPS_IM2COL_U8, OP_MAXPOOL3S2, OP_NHWC_TO_NCHW, OP_PIXEL_UNSHUFFLE_U8, OP_POSTPROCESS_U8,
+                    OP_SOFTMAX_ROWS, OP_UPSAMPLE_NEAREST, Op, check, ctx, stream_ptr)
 
 _DT16 = {torch.float16: _cabi.DTYPE_F16, torch.bfloat16: _cabi.DTYPE_BF16}   # the ops with fp16 and bf16 variants
 _TILING = {"auto": 0, "box": _cabi.GEMM_TILE_BOX, "runs": _cabi.GEMM_TILE_RUNS}
@@ -245,6 +245,39 @@ class Program:
         _same_dtype(x.dtype, "im2col_s2_pad01 x / out", out)
         d = self._new(OP_IM2COL_S2_PAD01).u.resample
         d.x, d.ld_x, d.B, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), B, H, W, C, _p(out), out.stride(0)
+        self.hold(x, out)
+
+    def add_rows_bcast(self, dst, src, B):
+        """fp16 ``dst[b*rows + r] += src[r]`` in place for every batch row b (lb_add_rows_bcast): ``dst`` [B*rows, C]
+        and ``src`` [rows, C], row-major with any row stride (a skip view inside a concat buffer, say)."""
+        _same_dtype(torch.float16, "add_rows_bcast dst / src", dst, src)
+        rows, C = src.shape
+        if tuple(dst.shape) != (B * rows, C):
+            raise _cabi.LB200Error(f"add_rows_bcast: dst {tuple(dst.shape)} is not {B} x src {tuple(src.shape)}")
+        d = self._new(OP_ADD_ROWS_BCAST).u.aux
+        d.out, d.ld_out, d.x, d.ld_x, d.B, d.n, d.C = _p(dst), dst.stride(0), _p(src), src.stride(0), B, rows, C
+        self.hold(dst, src)
+
+    def pixel_unshuffle_u8(self, img_u8, r, out):
+        """uint8 image [H, W, Cimg] -> fp16 ``out`` [(H/r)*(W/r), r*r*Cimg], u / 255, columns in (i, j, c) order
+        (lb_pixel_unshuffle_u8)."""
+        if img_u8.dtype != torch.uint8 or img_u8.dim() != 3 or not img_u8.is_contiguous():
+            raise _cabi.LB200Error(f"pixel_unshuffle_u8: the image must be a contiguous uint8 [H, W, C] tensor (got "
+                                   f"{img_u8.dtype} {tuple(img_u8.shape)})")
+        _same_dtype(torch.float16, "pixel_unshuffle_u8 out", out)
+        H, W, C = img_u8.shape
+        if tuple(out.shape) != ((H // r) * (W // r), r * r * C) or not out.is_contiguous():
+            raise _cabi.LB200Error(f"pixel_unshuffle_u8: out must be contiguous [{(H // r) * (W // r)}, {r * r * C}]")
+        d = self._new(OP_PIXEL_UNSHUFFLE_U8).u.patch
+        d.x, d.H, d.W, d.C, d.k, d.out, d.ld_out = _p(img_u8), H, W, C, r, _p(out), out.stride(0)
+        self.hold(img_u8, out)
+
+    def avgpool2_ceil(self, x, H, W, C, out):
+        """AvgPool2d(2, 2, ceil_mode=True) of the fp16 NHWC map ``x`` [H*W, >=C] into ``out`` [ceil(H/2)*ceil(W/2),
+        >=C] (lb_avgpool2_ceil)."""
+        _same_dtype(torch.float16, "avgpool2_ceil x / out", x, out)
+        d = self._new(OP_AVGPOOL2_CEIL).u.patch
+        d.x, d.ld_x, d.H, d.W, d.C, d.out, d.ld_out = _p(x), x.stride(0), H, W, C, _p(out), out.stride(0)
         self.hold(x, out)
 
     def latent_prep(self, x_nchw, w_f32, bias_f32, out_nchw):

@@ -168,14 +168,26 @@ class PackedUNet:
 class UNetB200:
     """One lowered forward per (batch, h, w); ``forward`` replays it."""
 
-    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0", controlnet=None):
+    def __init__(self, cfg: UNetConfig, state_dict, device="cuda:0", controlnet=None, adapter=None):
         """``controlnet``: a ``controlnet.ControlNetB200`` on the same device; every plan then also records
-        ``prog_step_cn``, the step with the ControlNet's residuals added."""
+        ``prog_step_cn``, the step with the ControlNet's residuals added.
+        ``adapter``: a ``t2i_adapter.AdapterB200`` on the same device; every plan whose size the adapter supports then
+        also records ``prog_step_ad``, the step with the adapter's four states added in the down path."""
+        if adapter is not None:
+            if controlnet is not None:
+                raise ValueError("a ControlNet and a T2I-Adapter together are not supported")
+            ch = tuple(cfg.block_out_channels)
+            if len(ch) != 3:
+                raise ValueError(f"a T2I-Adapter needs a UNet with 3 levels (this one has {len(ch)})")
+            if tuple(adapter.channels) != ch + ch[-1:]:
+                raise ValueError(f"the T2I-Adapter's channels {tuple(adapter.channels)} do not match the UNet's "
+                                 f"{ch + ch[-1:]} (block_out_channels, then the last one again)")
         self.cfg = cfg
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
         self.packed = PackedUNet(cfg, state_dict, self.device)
         self.controlnet = controlnet
+        self.adapter = adapter
         self._plans = {}
 
     # -- public -----------------------------------------------------------------------------
@@ -189,11 +201,12 @@ class UNetB200:
 
     @torch.no_grad()
     def forward(self, x, t, encoder_hidden_states, text_embeds, time_ids, ctx_changed=True, timestep_cond=None,
-                control=False):
+                control=False, adapter=False):
         """x [B,4,h,w] fp16 NCHW -> eps [B,4,h,w] fp16 (a view of the plan's static output buffer).
         ``timestep_cond`` [B, time_cond_proj_dim]: the guidance-scale embedding a time-conditioned UNet requires.
         ``control``: add the attached ControlNet's residuals (its conditioning embedding for (h, w) as last
-        filled by ``ControlNetB200.embed``, its scale as last set)."""
+        filled by ``ControlNetB200.embed``, its scale as last set).
+        ``adapter``: add the attached T2I-Adapter's states for (h, w) as last filled by ``AdapterB200.compute``."""
         B, _, H, W = x.shape
         pl = self.plan(B, H, W)
         if (pl.wcond is None) != (timestep_cond is None):
@@ -208,7 +221,9 @@ class UNetB200:
             pl.prog_ctx.run()
         if control and pl.prog_step_cn is None:
             raise ValueError("control=True needs a UNetB200 built with a controlnet")
-        (pl.prog_step_cn if control else pl.prog_step).run(float(t))
+        if adapter and pl.prog_step_ad is None:
+            raise ValueError("adapter=True needs a UNetB200 built with a T2I-Adapter, at a size it supports")
+        (pl.prog_step_cn if control else pl.prog_step_ad if adapter else pl.prog_step).run(float(t))
         return pl.eps
 
     def launches_per_forward(self, B, H, W):
@@ -335,11 +350,15 @@ class _Lowering:
                 P.gemm(gg, Wt[t + ".ff.out.w"], C, 1, 1, M, hs, bias=Wt[t + ".ff.out.b"], res=hs)
             P.gemm(hs, Wt[aname + ".proj_out.w"], C, 1, 1, M, out, bias=Wt[aname + ".proj_out.b"], res=x)
 
-        def down_mid(P, prm, dsts, mid_dst):
+        def down_mid(P, prm, dsts, mid_dst, marks=None):
             """The down path and the mid block of a net whose conv_in output is in ``dsts[0]``: each resnet /
             attention output and each downsampler output goes to the next of ``dsts`` (production order), the mid
             block's output to ``mid_dst``.  The UNet passes its concat-buffer skip views, a ControlNet its own
-            buffers; ``prm``: that net's packed weights, time-embedding projections and transformer depths."""
+            buffers; ``prm``: that net's packed weights, time-embedding projections and transformer depths.
+            ``marks`` (a list): appended with (op index, buffer) at each point where diffusers adds a
+            ``down_intrablock_additional_residuals`` state: a block with attention after its last resnet /
+            attention pair (before its downsampler), a block without after the whole block (its downsampler output,
+            which is also its last skip), and the mid block's output."""
             Wt = prm["W"]
             x, cin = dsts[0], ch[0]
             si = 1
@@ -356,6 +375,8 @@ class _Lowering:
                         resnet(P, prm, rname, x, cin, cout, i, dst)
                     x, cin = dst, cout
                     si += 1
+                if prm["depths"][i] and marks is not None:
+                    marks.append((len(P.ops), x))
                 if i < L - 1:
                     nm = f"down_blocks.{i}.downsamplers.0.conv"
                     h_, w_ = res_hw[i]
@@ -365,17 +386,22 @@ class _Lowering:
                     P.gemm(cols, Wt[nm + ".w"], cout, 1, 1, rows_at(i + 1), dst, bias=Wt[nm + ".b"])
                     x = dst
                     si += 1
+                if not prm["depths"][i] and marks is not None:
+                    marks.append((len(P.ops), x))
             lv, cm = L - 1, ch[-1]
             m1 = persist(rows_at(lv), cm)
             resnet(P, prm, "mid_block.resnets.0", x, cm, cm, lv, m1)
             m2 = persist(rows_at(lv), cm)
             transformer(P, prm, "mid_block.attentions.0", m1, cm, lv, m2)
             resnet(P, prm, "mid_block.resnets.1", m2, cm, cm, lv, mid_dst)
+            if marks is not None:
+                marks.append((len(P.ops), mid_dst))
         self.down_mid = down_mid
 
         # ---- down path + mid ------------------------------------------------------------------
         P.conv_in(self.x_in, Wt["conv_in.w"], Wt["conv_in.b"], ch[0], skip_views[0])
-        down_mid(P, unet, skip_views, cats[0]["hidden"])
+        marks = []              # where a T2I-Adapter's states are added (prog_step_ad)
+        down_mid(P, unet, skip_views, cats[0]["hidden"], marks)
         n_down_mid = len(P.ops)          # a ControlNet's records go here, after the UNet's mid block read its input
         # ---- up path ------------------------------------------------------------------------
         ci = 0
@@ -426,6 +452,23 @@ class _Lowering:
             self.prog_step_cn.ops = P.ops[:n_down_mid] + PX.ops + P.ops[n_down_mid:]
             self.prog_step_cn.keep = P.keep + PX.keep
             self.prog_step_cn.finalize()
+        # with a T2I-Adapter: the UNet's records with one in-place add of each adapter state spliced in at its mark
+        self.prog_step_ad = None
+        if net.adapter is not None and net.adapter.supports(H, W):
+            PA = Program(net.dev_index)
+            for k, ((_, buf), st) in enumerate(zip(marks, net.adapter.states(H, W))):
+                if tuple(buf.shape) != (B * st.shape[0], st.shape[1]):
+                    raise ValueError(f"the T2I-Adapter's state {k} {tuple(st.shape)} does not fit the UNet's injection "
+                                     f"point {tuple(buf.shape)} at batch {B}")
+                PA.add_rows_bcast(buf, st, B)
+            ops, prev = [], 0
+            for (idx, _), op in zip(marks, PA.ops):
+                ops += P.ops[prev:idx] + [op]
+                prev = idx
+            self.prog_step_ad = Program(net.dev_index)
+            self.prog_step_ad.ops = ops + P.ops[prev:]
+            self.prog_step_ad.keep = P.keep + PA.keep
+            self.prog_step_ad.finalize()
         P.finalize()
         PC.finalize()
 
